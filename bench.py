@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""bench.py -- benchmark of the B200 Paillier engine on the BASELINE.json configurations.
+"""bench.py -- benchmark of the H100 Paillier engine on the BASELINE.json configurations.
 
 Headline ("step"): raw_encrypt of a batch of 2048-bit-key plaintexts followed by raw_decrypt of the resulting
 ciphertexts (BASELINE.json configs[1]: 2048-bit key, batch 1M, bit-exact round trip).  `value` is encrypts/s of the
@@ -16,7 +16,13 @@ Extra keys of the same JSON line (each leg is outside the headline's timed regio
   federated        configs[4]: one round of the federated-learning example shape (rank 0, N = 1)
   reductions       EncryptedVector.sum / dot (fused kernels) against the launch chains they replace
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--impl reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--impl reference] [--dump-outputs DIR]
+
+`--steps K` sets the timed steps of the headline and of the raw_add / u64 raw_mul leg; the float-encoded and
+negative-scalar raw_mul mixes are timed once each, `e2e` runs min(K, --e2e-steps) steps and the 3072-bit leg one pass.
+`--dump-outputs DIR` writes, after the timed steps, what the headline's last step computed for a fixed sample of rows
+(sample_indices(batch, 4096, 1234)): DIR/ciphertext_limbs.npy and DIR/plaintext_limbs.npy, limbs as float64 (exact for
+32-bit limbs); the inputs are seeded, so two builds can be compared output for output.
 
 Multi-GPU (torchrun, one rank per GPU): the headline batch shards across ranks (weak scaling: `--batch` is the per-GPU
 batch), no data-path collective; the key limbs are broadcast from rank 0 over NCCL.
@@ -103,7 +109,7 @@ def executed_macs(kb, n=None, scalar_bits=64, enc_path="digit", dec_path="digit"
 
 
 def canonical_macs(kb, scalar_bits=64):
-    """SURVEY.md section 8(d): canonical 32x32->64 MAC counts (schoolbook CIOS, window 5, no squaring credit)."""
+    """Canonical 32x32->64 MAC counts (schoolbook CIOS, window 5, no squaring credit)."""
     def modmul(L):
         return 2 * L * L + L
 
@@ -330,37 +336,15 @@ def run_reference(args, key):
 def measured_int_peak():
     """Peak 32x32->64 MAC rate of the integer pipe, measured by bench_micro/imad_peak (IMAD.WIDE.U32.X chains)."""
     exe = os.path.join(ROOT, "bench_micro", "imad_peak")
-    fallback = {"mac_per_clk_sm": 25.1, "source": "profiles/r01_imad_peak.json (earlier measurement on this pool)"}
-    if not os.path.exists(exe):
-        return fallback
-    try:
-        out = subprocess.run([exe], capture_output=True, text=True, timeout=120).stdout
-        js = json.loads(out)
-        best = max((r for r in js["results"] if "wide_chain" in r["op"]), key=lambda r: r["thread_ops_per_clk_per_sm"])
-        res = {"mac_per_clk_sm": best["thread_ops_per_clk_per_sm"], "op": best["op"], "mhz": best["eff_mhz"], "sms": js["sms"],
-               "source": "bench_micro/imad_peak run inside this bench"}
-        noadd = [r for r in js["results"] if r["op"] == "mul_wide_no_addend"]
-        if noadd:
-            res["mul_wide_no_addend_per_clk_sm"] = max(r["thread_ops_per_clk_per_sm"] for r in noadd)
-        return res
-    except Exception as e:     # noqa: BLE001
-        fallback["error"] = str(e)[:100]
-        return fallback
-
-
-def _ncu_traffic(name):
-    """DRAM bytes (read + write) per row of the named kernel from the committed `ncu --set full` capture summary
-    (profiles/r02c_ncu_traffic.json: the final build; falling back to earlier captures)."""
-    for fn in ("r02c_ncu_traffic.json", "r02_ncu_traffic.json", "r01_ncu_traffic.json"):
-        try:
-            with open(os.path.join(ROOT, "profiles", fn)) as f:
-                t = json.load(f)
-            t = t.get(name, t) if isinstance(t.get(name), dict) else t
-            return {"bytes_per_ciphertext": t["bytes_per_ciphertext"], "algorithmic_bytes_per_ciphertext": 1024,
-                    "source": "profiles/" + fn + ": " + t.get("source", "")}
-        except (OSError, KeyError, ValueError, AttributeError):
-            continue
-    return None
+    out = subprocess.run([exe], capture_output=True, text=True, timeout=120, check=True).stdout
+    js = json.loads(out)
+    best = max((r for r in js["results"] if "wide_chain" in r["op"]), key=lambda r: r["thread_ops_per_clk_per_sm"])
+    res = {"mac_per_clk_sm": best["thread_ops_per_clk_per_sm"], "op": best["op"], "mhz": best["eff_mhz"], "sms": js["sms"],
+           "source": "bench_micro/imad_peak run inside this bench"}
+    noadd = [r for r in js["results"] if r["op"] == "mul_wide_no_addend"]
+    if noadd:
+        res["mul_wide_no_addend_per_clk_sm"] = max(r["thread_ops_per_clk_per_sm"] for r in noadd)
+    return res
 
 
 _OUT = None
@@ -493,7 +477,7 @@ def leg_headline(dev, args, pb, np, key, pool):
     dev.barrier()
     t_wall0 = time.perf_counter()
     for i in range(args.steps):
-        dev.l2_flush.zero_()                       # flush L2 between timed iterations (256 MiB > 126 MB L2)
+        dev.l2_flush.zero_()                       # flush L2 between timed iterations (256 MiB > 50 MB L2)
         ev[i][0].record()
         pub.encrypt_dev(d_m, d_r, d_c, B, stream=st)
         ev[i][1].record()
@@ -502,6 +486,11 @@ def leg_headline(dev, args, pb, np, key, pool):
     dev.barrier()
     t_wall = time.perf_counter() - t_wall0
     launches = eng.launch_count() - launches0
+    if args.dump_outputs and dev.rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        ti = torch.tensor(sample_indices(B, 4096, 1234), device="cuda")
+        for name, t in (("ciphertext_limbs", d_c[ti]), ("plaintext_limbs", d_d[ti])):
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), t.cpu().numpy().view(np.uint32).astype(np.float64))
     enc_each = sorted(e[0].elapsed_time(e[1]) for e in ev)
     dec_each = sorted(e[1].elapsed_time(e[2]) for e in ev)
     spread = {"encrypt_ms": {"min": enc_each[0], "median": enc_each[len(enc_each) // 2], "max": enc_each[-1]},
@@ -580,7 +569,7 @@ def leg_add_mul(dev, args, pb, np, key, pool, state, peak_mac_s):
     d_o = torch.empty_like(d_c)
     status = torch.zeros((B,), dtype=torch.int32, device="cuda")
     out = {"batch_per_gpu": B}
-    steps = max(1, min(args.steps, 3))
+    steps = args.steps
     pub.raw_add_dev(d_c, d_c2, d_o, B, stream=st)
     add_ms = dev.timed(lambda: pub.raw_add_dev(d_c, d_c2, d_o, B, stream=st), steps)
     priv.decrypt_dev(d_o, d_d, B, stream=st)
@@ -648,10 +637,7 @@ def leg_add_mul(dev, args, pb, np, key, pool, state, peak_mac_s):
 
 
 def _hbm_peak():
-    peaks_file = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(peaks_file):
-        return json.load(open(peaks_file))["hbm_gbs"], "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3), not measured"
 
 
 def leg_3072(dev, args, pb, np, pool, peak_mac_s, H, load_golden):
@@ -772,7 +758,7 @@ def leg_multi_parity(dev, args, pb, np, pool, H, load_golden):
 
 
 def leg_reductions(dev, args, pb, np, key, pool, state):
-    """SURVEY 8(f2): homomorphic sum / dot of a 1e5-element encrypted vector, fused kernels vs the launch chains."""
+    """Homomorphic sum / dot of a 1e5-element encrypted vector, fused kernels vs the launch chains."""
     torch = dev.torch
     vec = __import__("importlib").import_module("python-paillier_b200.vector")
     if not hasattr(vec.EncryptedVector, "sum_chain"):
@@ -898,6 +884,7 @@ def main():
     ap.add_argument("--reduce-rows", type=int, default=100000)
     ap.add_argument("--fed-dim", type=int, default=100000)
     ap.add_argument("--fed-cpu-sample", type=int, default=60)
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write a seeded sample of the headline's last-step outputs as .npy")
     args = ap.parse_args()
     # the contract is ONE JSON line on stdout: native libraries (NCCL's version banner, ...) write to fd 1 as well, so
     # everything but the final line is sent to stderr
@@ -933,11 +920,12 @@ def main():
     enc_per_s = world * B / (enc_ms * 1e-3)
     dec_per_s = world * B / (dec_ms * 1e-3)
     clocks = head["clocks"]
-    peak = measured_int_peak() if dev.rank == 0 else {"mac_per_clk_sm": 25.1}
-    sm_mhz = (clocks or {}).get("sm_mhz") or peak.get("mhz") or 1965.0
+    peak = measured_int_peak() if dev.rank == 0 else {"mac_per_clk_sm": 0.0}
+    sm_mhz = (clocks or {}).get("sm_mhz") or peak.get("mhz")
     (pk_mac, sm_mhz) = dev.max_over_ranks([peak["mac_per_clk_sm"] if dev.rank == 0 else 0.0, sm_mhz if dev.rank == 0 else 0.0])
-    peak_mac_s = pk_mac * 148 * sm_mhz * 1e6
-    nominal_mac_s = NOMINAL_MAC_PER_CLK_SM * 148 * sm_mhz * 1e6
+    sms = dev.torch.cuda.get_device_properties(dev.local).multi_processor_count
+    peak_mac_s = pk_mac * sms * sm_mhz * 1e6
+    nominal_mac_s = NOMINAL_MAC_PER_CLK_SM * sms * sm_mhz * 1e6
 
     extras = {}
     if not args.no_extras:
@@ -966,10 +954,10 @@ def main():
     ex, ca = executed_macs(KEY_BITS, key[0], enc_path=head["enc_path"], dec_path=head["dec_path"]), canonical_macs(KEY_BITS)
     hbm_peak, hbm_src = _hbm_peak()
     ach = enc_per_s / world * ex["encrypt"]
-    kern = {"tc": "k_body<TcEncBody<8>> (raw_encrypt: digit products on the integer pipe, Montgomery reductions as tcgen05 kind::i8 GEMMs)",
+    kern = {"tc": "k_body<TcEncBody<8>> (raw_encrypt: digit products on the integer pipe, Montgomery reductions as wgmma u8 GEMMs)",
             "digit": "k_body<EncDigitBody<8>> (raw_encrypt, r^n mod n^2 on base-n digits)", "full": "k_body<EncBody<16>>"}
     kern_d = {"tc": "k_body<TcDecBody<4,5>>", "digit": "k_body<DecDigitBody<4,5>>", "full": "k_body<DecBody<4,5>>"}
-    tensor_peak = 2 * json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["bf16_tflops"] / 2 if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 1590.0
+    tensor_peak = 1979.0 / 2                        # H100 SXM data sheet: 1,979 dense 8-bit TOP/s = 989.5 T MAC/s
     roofline = {
         "bound": "int_pipe", "kernel": kern[head["enc_path"]], "kernel_family": head["enc_path"],
         "achieved": ach / 1e12, "peak": peak_mac_s / 1e12, "unit": "TMAC/s (32x32->64 MACs the kernel executes, per GPU)",
@@ -977,25 +965,24 @@ def main():
         "frac_of_nominal_pipe": ach / nominal_mac_s, "peak_nominal": nominal_mac_s / 1e12,
         "canonical_frac": enc_per_s / world * ca["encrypt"] / peak_mac_s,
         "executed_macs_per_encrypt": ex["encrypt"], "canonical_macs_per_encrypt": ca["encrypt"],
-        "note": "frac = MACs executed on the integer pipe / measured IMAD.WIDE.U32 peak.  canonical_frac uses SURVEY 8(d)'s schoolbook count; the "
+        "note": "frac = MACs executed on the integer pipe / measured IMAD.WIDE.U32 peak.  canonical_frac uses the schoolbook count (canonical_macs); the "
                 "base-n digit arithmetic halves it and the tensor-core reductions halve it again (algorithmic savings, not throughput) -- "
                 "it exceeds 1.  peak_nominal = 32 MAC/clk/SM "
                 "(half-rate fmaheavy instruction); the measured peak is ~25: an IMAD.WIDE with a 64-bit addend issues every 5th cycle "
                 "per SM sub-partition, not every 4th (bench_micro/imad_peak: the same instruction without an addend, "
                 "mul_wide_no_addend, is reported beside it), so ~0.78 of nominal is the ceiling of this instruction and ncu's "
                 "sm__pipe_fmaheavy_cycles_active tops out near 80 %",
-        "peak_source": "measured IMAD.WIDE.U32.X rate %.1f MAC/clk/SM (%s) x 148 SMs x %.0f MHz (SM clock sampled under load)"
-                       % (pk_mac, peak.get("source"), sm_mhz),
+        "peak_source": "measured IMAD.WIDE.U32.X rate %.1f MAC/clk/SM (%s) x %d SMs x %.0f MHz (SM clock sampled under load)"
+                       % (pk_mac, peak.get("source"), sms, sm_mhz),
         "peak_micro": peak,
         "decrypt": {"kernel": kern_d[head["dec_path"]], "kernel_family": head["dec_path"], "frac": dec_per_s / world * ex["decrypt"] / peak_mac_s,
                     "canonical_frac": dec_per_s / world * ca["decrypt"] / peak_mac_s, "executed_macs_per_decrypt": ex["decrypt"]},
         "tensor": {"u8_macs_per_encrypt": ex["encrypt_tensor_u8_macs"], "achieved_tmacs": enc_per_s / world * ex["encrypt_tensor_u8_macs"] / 1e12,
                    "peak_tmacs_int8_dense": tensor_peak, "frac": enc_per_s / world * ex["encrypt_tensor_u8_macs"] / 1e12 / tensor_peak,
-                   "note": "the reductions' GEMMs ([128 x D] x Toeplitz, u8 x u8 -> s32); peak = measured dense bf16 TFLOP/s x 2 (int8) / 2 (MAC = 2 ops); "
+                   "note": "the reductions' GEMMs ([128 x D] x Toeplitz, u8 x u8 -> s32); peak = data-sheet dense 8-bit TOP/s / 2 (MAC = 2 ops); "
                            "the tensor pipe is a helper here, not the bound"},
         "hbm": {"achieved_gbs": enc_per_s / world * (ln * 2 + lc) * 4 / 1e9, "peak_gbs": hbm_peak, "peak_source": hbm_src,
                 "frac": enc_per_s / world * (ln * 2 + lc) * 4 / 1e9 / hbm_peak},
-        "traffic": _ncu_traffic("encrypt"),
     }
     cpu = None
     if pool is not None and world == 1:

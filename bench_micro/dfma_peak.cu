@@ -1,10 +1,10 @@
-// FP64-pipe big-integer product microbenchmark for sm_100a.
+// FP64-pipe big-integer product microbenchmark for sm_90a.
 // A 52x52 -> 104-bit product as two round-toward-zero DFMAs and one DADD (the double-precision split used by
 // Emmart, Zheng & Weems, ARITH 2018):  hi = fma_rz(a, b, 2^104), lo = fma_rz(a, b, (2^104 + 2^52) - hi); the bit
 // patterns of hi / lo carry the high / low 52 bits of a*b in their mantissas and are summed as 64-bit integers.
 // Measures products / clk / SM of an 8x8-limb tile product (64 products into 16 column sums) in the
 // thread-per-element form the Paillier kernels use, against the 25.1 MAC(32x32)/clk/SM of the IMAD.WIDE carry chains.
-//   build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o dfma_peak dfma_peak.cu
+//   build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o dfma_peak dfma_peak.cu
 #include <cstdint>
 #include <cstdio>
 #include <cuda_runtime.h>

@@ -1,7 +1,7 @@
-// Integer-pipe microbenchmark for sm_100a: measures the sustained issue rate of the
+// Integer-pipe microbenchmark for sm_90a: measures the sustained issue rate of the
 // instructions the Montgomery kernels are built from, so that roofline.peak in bench.py
 // is a MEASURED number, not the nominal 64 IMAD/clk/SM.
-//   build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o imad_peak imad_peak.cu
+//   build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o imad_peak imad_peak.cu
 //   run  : ./imad_peak            (prints one JSON object)
 #include <cstdint>
 #include <cstdio>

@@ -19,8 +19,8 @@ fx = load_golden("vectors_%d.json" % kb)
 n, p, q = H(fx["n"]), H(fx["p"]), H(fx["q"])
 pub, priv = pkg.PublicContext(n), pkg.PrivateContext(p, q)
 rng = np.random.default_rng(0)
-sizes = [1, 8, 64, 148, 592, 1024, 2368, 4736, 9472]
-hybrid = 33152 + 4000            # one full encrypt wave at 2048 bit plus a tail
+sizes = [1, 8, 64, 132, 528, 1024, 2112, 4224, 8448]
+hybrid = pub.wave() + 4000       # one full encrypt wave plus a tail
 top = max(sizes + [hybrid])
 m = rng.integers(0, 2 ** 32, size=(top, pub.n_limbs), dtype=np.uint32); m[:, kb // 32 - 1:] = 0
 r = rng.integers(0, 2 ** 32, size=(top, pub.n_limbs), dtype=np.uint32); r[:, kb // 32 - 1:] = 0; r[:, 0] |= 1
@@ -32,7 +32,7 @@ ref = None
 for mode, env in (("thread", "0"), ("warp", "1000000")):
     os.environ["PAI_COOP_MAX"] = env
     for b in sizes:
-        if mode == "thread" and b not in (1, 148, 1024, 9472):
+        if mode == "thread" and b not in (1, 132, 1024, 8448):
             continue
         for _ in range(2):
             pub.encrypt_dev(d_m, d_r, d_c, b); priv.decrypt_dev(d_c, d_d, b)

@@ -1,5 +1,5 @@
-// Microbenchmark: sustained rate of the tile Montgomery square / multiply (pai_core.cuh) on sm_100a.
-//   build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -o mont_rate mont_rate.cu
+// Microbenchmark: sustained rate of the tile Montgomery square / multiply (pai_core.cuh) on sm_90a.
+//   build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -o mont_rate mont_rate.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>

@@ -11,7 +11,7 @@ kb = 2048
 fx = load_golden("vectors_%d.json" % kb)
 n = H(fx["n"])
 pub = pb.PublicContext(n); priv = pb.PrivateContext(H(fx["p"]), H(fx["q"]))
-batch = 148 * 224
+batch = 132 * 224
 ln, lc = pub.n_limbs, pub.c_limbs
 rng = np.random.default_rng(1)
 m = rng.integers(0, 2**32, size=(batch, ln), dtype=np.uint32); m[:, kb // 32 - 1:] = 0

@@ -38,5 +38,5 @@ def run(kb, batch):
     print(json.dumps(res), flush=True)
 
 if __name__ == "__main__":
-    for kb, b in [(1024, 148 * 256 * 4), (2048, 148 * 224 * 4), (3072, 148 * 128 * 2)]:
+    for kb, b in [(1024, 132 * 256 * 4), (2048, 132 * 224 * 4), (3072, 132 * 128 * 2)]:
         run(kb, b)

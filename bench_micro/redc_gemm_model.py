@@ -1,5 +1,5 @@
-"""Numerical model (numpy, CPU) of the next-round kernel idea in DESIGN.md section 8: the two constant-operand
-multiplications of a Montgomery reduction as batch GEMMs in 8-bit digits -- the arithmetic a `tcgen05.mma kind::i8`
+"""Numerical model (numpy, CPU) of the reductions of pai_tc.cuh: the two constant-operand
+multiplications of a Montgomery reduction as batch GEMMs in 8-bit digits -- the arithmetic a u8 x u8 -> s32 tensor-core (`wgmma`)
 kernel would perform, with the int32 column-sum bounds checked.  Not used by the engine; exercised by
 tests/test_redc_gemm_model.py against Python integers.
 

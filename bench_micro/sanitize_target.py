@@ -1,7 +1,7 @@
 """Small workload for compute-sanitizer (memcheck / racecheck): every round-2 kernel on a 1024-bit key -- tensor-core
 encrypt / decrypt / raw_mul (forced: PAI_TC=2), amortised inversion, product reduction, Straus dot product, batched
 Miller-Rabin, and the same context driven from two CUDA streams.   python sanitize_target.py [rows [key_bits]]
-(2048-bit keys with PAI_TC_GROUPS=3 in the environment: three groups per CTA sharing two TMEM accumulators, x1 in L2)"""
+(2048-bit keys with PAI_TC_GROUPS=3 in the environment: three groups per CTA, x1 in L2)"""
 import os, sys
 os.environ["PAI_TC"] = "2"
 os.environ["PAI_COOP_MAX"] = "0"

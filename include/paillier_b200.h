@@ -1,5 +1,5 @@
 /*
- * paillier_b200.h -- C ABI of the B200-native batched Paillier engine (libpaillier_b200.so).
+ * paillier_b200.h -- C ABI of the H100-native batched Paillier engine (libpaillier_b200.so).
  *
  * This is the drop-in boundary for the big-integer hot path of data61/python-paillier (phe 1.5.0).
  * The reference reaches its bigint engine (gmpy2 -> GMP) through three scalar functions,
@@ -26,8 +26,8 @@
  *   - Batch size needs no tuning: pai_encrypt / pai_decrypt / pai_mod_powmod_shared route a batch (or the remainder of
  *     a batch beyond whole waves of the thread-per-ciphertext kernels) of up to 0.3 wave to warp-per-ciphertext
  *     kernels with ~10x lower latency.  Environment switches, read at call time / context creation:
- *     PAI_COOP_MAX=<rows> (0 = never use the warp kernels), PAI_TC=0 (base-n digit kernels on the integer pipe instead of
- *     the tensor-core reductions; 2 = tensor-core kernels for every size they exist for, default: digit moduli >= 1024 bits),
+ *     PAI_COOP_MAX=<rows> (0 = never use the warp kernels), PAI_TC=2 (the tensor-core reductions for every size they exist
+ *     for instead of the default base-n digit kernels on the integer pipe, which measure faster on the H100),
  *     PAI_TC_GROUPS=<1..4> (cap on the 128-thread groups per CTA of the tensor-core kernels; experiments and sanitizer runs),
  *     PAI_ENCRYPT_PATH=full, PAI_DECRYPT_PATH=full (full-width Montgomery kernels instead of the base-n digit kernels).
  *     All variants return identical bits.
@@ -87,8 +87,8 @@ int pai_pub_c_limbs(const pai_pub* k);     /* 2*Ln: limbs of ciphertexts        
 long pai_pub_wave(pai_pub* k);
 /* kernel family that serves pai_encrypt for this key: 0 = full-width Montgomery, 1 = base-n digit arithmetic on the
  * integer pipe (pai_digit.cuh), 2 = base-n digits with both multiplications of every Montgomery reduction on the
- * tensor cores (pai_tc.cuh; keys up to 3072 bits).  All families return identical bits; PAI_TC=0 / PAI_ENCRYPT_PATH=full
- * at context creation select the lower ones.  Instrumentation only (bench.py reports the MACs of the active family). */
+ * tensor cores (pai_tc.cuh; keys up to 3072 bits).  All families return identical bits; PAI_TC=2 / PAI_ENCRYPT_PATH=full
+ * at context creation select family 2 / 0 instead of the default 1.  Instrumentation only (bench.py reports the MACs of the active family). */
 int pai_pub_kernel_path(const pai_pub* k);
 
 /* c[i] = (1 + n*m[i]) * r[i]^n mod n^2        raw_encrypt, phe/paillier.py:102-139
@@ -145,7 +145,7 @@ int pai_limbs_to_decimal(const uint32_t* d_limbs, int limbs, uint8_t* d_text, lo
 int pai_decimal_to_limbs(const uint8_t* d_text, int width, uint32_t* d_limbs, int limbs, int32_t* d_status, long batch, int device,
                          void* stream);
 
-/* ---- batched primality testing for key generation (SURVEY.md 8f rank 4) ------------------------------------------
+/* ---- batched primality testing for key generation ----------------------------------------------------------
  * result[i] = 1 if candidate i passes `rounds` Miller-Rabin rounds with the bases given, 0 if it is composite:
  * util.miller_rabin (phe/util.py:381-417) for a whole batch of candidates, one thread per candidate, each with its own
  * Montgomery constants.  The reference's getprimeover / is_prime (phe/util.py:106-124, 420-443) test one candidate at a

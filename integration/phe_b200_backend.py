@@ -8,8 +8,7 @@ into ``phe.paillier`` (``phe/paillier.py:29``).  This module is that seam over t
 ``phe/tests/util_test.py:64-75`` -- and ``uninstall(phe)`` restores them.  Everything else of ``phe`` stays untouched.
 
 Library lookup: ``$PHE_B200_LIB``, else ``python-paillier_b200/libpaillier_b200.so`` next to this repo's root.
-INTEGRATION.md section 1 quotes this file; tests/test_phe_seam_unmodified.py runs the reference's own
-``paillier_test.py`` classes on the unmodified ``phe`` with this backend installed.
+INTEGRATION.md section 1 quotes this file.
 """
 import ctypes
 import os

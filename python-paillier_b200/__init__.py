@@ -1,4 +1,4 @@
-"""python-paillier_b200: a B200-native batched Paillier engine behind the ``phe`` API.
+"""python-paillier_b200: an H100-native batched Paillier engine behind the ``phe`` API.
 
 The directory name carries a hyphen (it mirrors the reference repo's name), so import it with
 ``importlib.import_module("python-paillier_b200")`` or through the root-level alias module

@@ -1,7 +1,7 @@
-"""Build the CUDA engine in-tree:  python-paillier_b200/libpaillier_b200.so  (sm_100a only).
+"""Build the CUDA engine in-tree:  python-paillier_b200/libpaillier_b200.so  (sm_90a only).
 
 nvcc cross-compiles without a GPU.  The .so is git-ignored but travels to the GPU box with the
-repo snapshot.  Rebuilds only when a source is newer than the library.
+repo snapshot.  Rebuilds only when a source or this file is newer than the library.
 """
 import os
 import shutil
@@ -13,7 +13,8 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libpaillier_b200.so")
 SOURCES = ["pai_engine.cu"]
 HEADERS = ["pai_core.cuh", "pai_kernels.cuh", "pai_digit.cuh", "pai_cta.cuh", "pai_coop.cuh", "pai_tc.cuh", "pai_rng.cuh", "pai_radix.cuh", "pai_rt.h", os.path.join("..", "..", "include", "paillier_b200.h")]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+# --split-compile 0: the device optimisation of the many kernel instantiations runs on every host core
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "--split-compile", "0",
               "-Xcompiler", "-fPIC", "-shared", "-Xptxas", "-v"]
 
 
@@ -25,10 +26,13 @@ def find_nvcc():
 
 
 def needs_build():
+    """True when the library is missing or older than a source or than this file (which holds the flags and the target
+    architecture)."""
     if not os.path.exists(LIB):
         return True
     t = os.path.getmtime(LIB)
-    return any(os.path.getmtime(os.path.join(CSRC, f)) > t for f in SOURCES + HEADERS)
+    deps = [os.path.join(CSRC, f) for f in SOURCES + HEADERS] + [os.path.abspath(__file__)]
+    return any(os.path.getmtime(d) > t for d in deps)
 
 
 def build(force=False, verbose=False):

@@ -1,13 +1,13 @@
-// pai_core.cuh -- multi-precision primitives of the B200 Paillier engine.
+// pai_core.cuh -- multi-precision primitives of the H100 Paillier engine.
 //
 // One THREAD owns one big integer ("instance").  Numbers are little-endian arrays of 32-bit limbs
 // grouped in TILES of 8 limbs (256 bit).  Operands live in shared memory in an interleaved layout
 // (quad q of thread t at  base[q * nthreads + t], 16 bytes each) so that every LDS.128/STS.128 of
 // a warp is conflict free; tile products run in registers as chains of IMAD.WIDE.U32(.X) that
-// ptxas fuses from  mad.lo.cc / madc.hi.cc  pairs (verified with cuobjdump on sm_100a).
+// ptxas fuses from  mad.lo.cc / madc.hi.cc  pairs (verified with cuobjdump on sm_90a).
 //
 // Everything in this header is written once and compiled twice:
-//   * by nvcc for sm_100a (the product), and
+//   * by nvcc for sm_90a (the product), and
 //   * by g++ with -DPAI_HOSTSIM (tests/hostsim: a TEST-ONLY build that runs the very same
 //     templates on the CPU, one simulated thread at a time, so the algorithms can be checked
 //     against the oracle in the GPU-less build container).  The product never loads that build.

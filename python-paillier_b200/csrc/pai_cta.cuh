@@ -150,24 +150,9 @@ template <int NTH>
 PAI_HD size_t tc_pow_smem_bytes(int nthr) { return tc_smem_bytes<NTH>(dc_pow_limbs(NTH), 2, nthr); }
 template <int NTP>
 PAI_HD size_t tc_dec_smem_bytes(int nthr) { return tc_smem_bytes<NTP>((2 * (dside_limbs<NTP>() / 4) + 2 * NTP) * 4, 4, nthr); }
-// accumulator slots of D = 32*NTH columns in the 512 TMEM columns of an SM
-PAI_HD int tc_tmem_slots(int NTH) { int n = 512 / (32 * NTH); return n < 1 ? 1 : (n > 4 ? 4 : n); }
-// columns to allocate for `groups` groups: all 512 when the groups share slots, else the next power of two
-template <int NTH>
-#if !defined(PAI_HOSTSIM)
-__host__ __device__
-#endif
-constexpr int tc_tmem_cols(int groups) {
-  int slots = 512 / (32 * NTH);
-  if (groups > slots) return 512;
-  int need = groups * 32 * NTH, c = 32;
-  while (c < need && c < 512) c *= 2;
-  return c;
-}
-
-// Set-up shared by the tensor-core kernels: copies the bands to shared memory, allocates TMEM and the groups' mbarriers,
-// fills in the context of the calling thread.  Returns the shared-memory address of the bands.  `entries`: user table
-// entries per thread; three more follow: the park slot and (tc_x1_global) the home of the high digit x1 and the W slot.
+// Set-up shared by the tensor-core kernels: copies the bands to shared memory and fills in the context of the calling
+// thread.  Returns the shared-memory address of the bands.  `entries`: user table entries per thread; three more follow:
+// the park slot and (tc_x1_global) the home of the high digit x1 and the W slot.
 template <int NTH>
 PAI_DEV uint8_t* tc_cta_begin(TcCtx<NTH>& c, u4* smem, const CtaId& id, int const_limbs, int nbands, const uint8_t* gbands, u4* tbl,
                               int entries, int stagger_cycles) {
@@ -201,68 +186,31 @@ PAI_DEV uint8_t* tc_cta_begin(TcCtx<NTH>& c, u4* smem, const CtaId& id, int cons
   c.tbl.s = id.nthr;
   (void)stagger_cycles;
 #else
-  __shared__ uint64_t s_mbar[4];
-  __shared__ uint32_t s_tmem;
-  __shared__ uint32_t s_locks[8];
-  const int groups = id.nthr / TC_M;
   {
     const u4* src = (const u4*)gbands;
     u4* dst = (u4*)bands;
     for (int i = id.tid; i < nbands * tc_band_bytes(NTH) / 16; i += id.nthr) dst[i] = src[i];
   }
-  if (id.tid == 0) { for (int i = 0; i < 4; i++) tc_mbar_init(&s_mbar[i], 1); for (int i = 0; i < 8; i++) s_locks[i] = 0; }
-  if (id.tid < 32) {
-    if (groups == 4) asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc_smem_u32(&s_tmem)), "n"(tc_tmem_cols<NTH>(4)));
-    else if (groups == 3) asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc_smem_u32(&s_tmem)), "n"(tc_tmem_cols<NTH>(3)));
-    else if (groups == 2) asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc_smem_u32(&s_tmem)), "n"(tc_tmem_cols<NTH>(2)));
-    else asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc_smem_u32(&s_tmem)), "n"(tc_tmem_cols<NTH>(1)));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");         // the bands are wgmma operands
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const int grp = id.tid / TC_M;
+  const int grp = id.tid / TC_M, lane = id.tid & 31;
   c.grp = grp;
-  c.ngroups = groups;
-  c.nslots = tc_tmem_slots(NTH);
-  c.locks = s_locks;
-  c.slot = grp;
+  c.which = 0;
   c.A = (u4*)(A0 + (size_t)grp * TC_M * D);
   c.tid = id.tid;
-  c.row0 = id.tid % TC_M;
-  c.tmem_base = s_tmem;
-  c.tmem = s_tmem + (uint32_t)((groups > c.nslots ? 0 : grp) * D);
-  c.mbar = &s_mbar[grp];
-  c.phase = 0;
+  // the row of the group whose column sums tc_ld32 brings to this lane: row (lane & 15) of this warp's 16 in m64 half lane >> 4
+  c.row0 = 64 * (lane >> 4) + 16 * ((id.tid % TC_M) >> 5) + (lane & 15);
   c.prof = nullptr;
   c.tbl.p = tbl + (size_t)id.cta * tbl_cta + id.tid;
   c.tbl.s = id.nthr;
   if (grp > 0 && stagger_cycles > 0) {                 // put the groups out of phase: some multiply while the others reduce
     const long long t0 = clock64();
-    while (clock64() - t0 < (long long)stagger_cycles * grp / groups * 2) {}
+    while (clock64() - t0 < (long long)stagger_cycles * grp / (id.nthr / TC_M) * 2) {}
   }
 #endif
   if (x1_global) c.H1 = tc_tbl<NTH>(c, entries + 1, 0, 0);
   else { c.H1.p = H1s + c.tid; c.H1.s = id.nthr; }
   return bands;
-}
-template <int NTH>
-PAI_DEV void tc_cta_end(const TcCtx<NTH>& c, const CtaId& id) {
-#if !defined(PAI_HOSTSIM)
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (id.tid < 32) {
-    const uint32_t t0 = c.tmem_base;
-    const int groups = id.nthr / TC_M;
-    if (groups == 4) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(t0), "n"(tc_tmem_cols<NTH>(4)));
-    else if (groups == 3) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(t0), "n"(tc_tmem_cols<NTH>(3)));
-    else if (groups == 2) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(t0), "n"(tc_tmem_cols<NTH>(2)));
-    else asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(t0), "n"(tc_tmem_cols<NTH>(1)));
-  }
-#else
-  (void)c; (void)id;
-#endif
 }
 // rows of this thread (simulation: of the TC_RL rows of the CTA) in chunk `chunk`
 PAI_DEV void tc_chunk_rows(const CtaId& id, long chunk, long batch, long* g, bool* store) {
@@ -292,7 +240,6 @@ PAI_DEV void cta_encrypt_tc(u4* smem, const CtaId& id, const uint32_t* prog, int
     tc_chunk_rows(id, chunk, batch, g, store);
     tc_encrypt_rows<NTH>(c, prog, nops, nodd, m, r, out, g, store);
   }
-  tc_cta_end<NTH>(c, id);
 }
 
 // ---- c^k mod n^2 (raw_mul) on the tensor-core path.  consts = compact constants with ONEM and E3 (dc_pow_limbs); the
@@ -324,7 +271,6 @@ PAI_DEV void cta_powmod_tc(u4* smem, const CtaId& id, const uint32_t* base, cons
 #endif
     tc_powmod_rows<NTH, W>(c, base, exp, exp_limbs, nwin, out, g, store);
   }
-  tc_cta_end<NTH>(c, id);
 }
 
 // ---- prod_i c_i^(k_i) over groups of gsz elements per thread (Straus, tc_straus_rows): one output row per group.
@@ -363,7 +309,6 @@ PAI_DEV void cta_straus_tc(u4* smem, const CtaId& id, const uint32_t* base, cons
 #endif
     tc_straus_rows<NTH, W>(c, base, exp, exp_limbs, gsz, nwin, batch, out, g, store);
   }
-  tc_cta_end<NTH>(c, id);
 }
 
 // ---- decrypt with the reductions on the tensor cores.  consts = [ P side | Q side | pinvqM ] as in cta_decrypt_digit;
@@ -383,7 +328,6 @@ PAI_DEV void cta_decrypt_tc(u4* smem, const CtaId& id, int nwin_p, int nwin_q, c
     tc_chunk_rows(id, chunk, batch, g, store);
     tc_decrypt_rows<NTP, W>(c, P, Qs, pinvqM, bands, cin, out, g, store);
   }
-  tc_cta_end<NTP>(c, id);
 }
 
 // ---- mulmod.  consts = [ blob ]

@@ -1,6 +1,6 @@
 // pai_engine.cu -- host orchestration + C ABI of libpaillier_b200.so (see include/paillier_b200.h).
 //
-// Product build:   nvcc -gencode arch=compute_100a,code=sm_100a ... -shared  (python-paillier_b200/build.py)
+// Product build:   nvcc -gencode arch=compute_90a,code=sm_90a ... -shared  (python-paillier_b200/build.py)
 // Test-only build: g++ -x c++ -DPAI_HOSTSIM ...  -> tests/hostsim/libpaillier_b200_hostsim.so
 //                  (same orchestration, kernels run on the CPU; never loaded by the product package)
 //
@@ -245,7 +245,7 @@ struct LBody {
 }  // namespace
 #if !defined(PAI_HOSTSIM)
 // tensor-core kernels of digit moduli with at most 4 tiles (128 base-256 digits: 2048-bit-key decrypt, 1024-bit-key encrypt)
-// keep 3 x 128 bytes per thread in shared memory, so FOUR 128-thread groups fit an SM (4 x 128 TMEM columns = all 512):
+// keep 3 x 128 bytes per thread in shared memory, so FOUR 128-thread groups fit an SM:
 // 16 warps instead of 8 to keep the integer pipe busy while other groups wait for their GEMMs -- at 128 registers a thread
 namespace pai {
 template <int W> struct BodyMaxThreads<TcDecBody<2, W>> { static const int v = 512; };
@@ -257,7 +257,7 @@ template <int W> struct BodyMaxThreads<TcPowBody<4, W>> { static const int v = 5
 template <int W> struct BodyMaxThreads<TcStrausBody<2, W>> { static const int v = 512; };
 template <int W> struct BodyMaxThreads<TcStrausBody<4, W>> { static const int v = 512; };
 // 192 / 256 digits: THREE groups (384 threads, 168 registers) once the high digit x1 lives in the thread's table strip in
-// L2 instead of shared memory; at 256 digits they share the two 256-column TMEM accumulators (taken per reduction)
+// L2 instead of shared memory
 template <int W> struct BodyMaxThreads<TcDecBody<6, W>> { static const int v = 384; };
 template <int W> struct BodyMaxThreads<TcDecBody<8, W>> { static const int v = 384; };
 template <> struct BodyMaxThreads<TcEncBody<6>> { static const int v = 384; };
@@ -459,7 +459,7 @@ struct pai_pub {
   uint32_t* d_enc_consts = nullptr; // compact constant area of the encrypt kernel (dc_enc_limbs)
   bool use_digit = true;            // PAI_ENCRYPT_PATH=full selects the full-width Montgomery path instead
   uint8_t* d_tc = nullptr;          // tensor-core path: [ band(N') | band(n) ] (pai_tc.cuh); null when not supported
-  bool use_tc = false;              // PAI_TC=0 disables it
+  bool use_tc = false;              // PAI_TC=2 enables it
   int tc_stagger = 0;               // start-up delay (cycles) of the second thread group
   long wave = 0;                    // ciphertexts per wave of the throughput encrypt kernel (lazily measured)
 };
@@ -543,14 +543,11 @@ namespace {
 
 // tile counts the tensor-core kernels are instantiated for (DISPATCH_TC), up to `max_tiles`
 bool tc_supported(int tiles, int max_tiles) { return (tiles == 2 || tiles == 4 || tiles == 6 || tiles == 8 || tiles == 12) && tiles <= max_tiles; }
-// PAI_TC: "0" never, "2" whenever the kernels exist, otherwise (default) where they were measured to win: encrypt for digit
-// moduli n of at least 4 tiles (1024-bit keys and up), decrypt for primes of at least 2 tiles (1024-bit keys and up; with
-// four 128-thread groups per SM: 3.73 M/s against 3.17 M/s on the integer pipe at 1024-bit keys)
-bool tc_wanted(int tiles, int min_tiles) {
+// PAI_TC=2 selects the tensor-core kernels wherever they exist; by default the integer-pipe digit kernels run, which
+// measure faster on the H100 at every key size both families cover (DESIGN.md section 4)
+bool tc_wanted() {
   const char* e = getenv("PAI_TC");
-  if (e && std::string(e) == "0") return false;
-  if (e && std::string(e) == "2") return true;
-  return tiles >= min_tiles;
+  return e && std::string(e) == "2";
 }
 
 template <int NT>
@@ -734,7 +731,7 @@ int do_encrypt_digit(pai_pub* k, const uint32_t* m_, const uint32_t* r, uint32_t
 }
 
 // launch geometry of a tensor-core kernel: as many 128-thread groups per CTA as the body's register budget
-// (BodyMaxThreads), shared memory (tc_x1_global decides where the high digit lives) and the TMEM accumulator slots allow.
+// (BodyMaxThreads) and shared memory (tc_x1_global decides where the high digit lives) allow.
 // PAI_TC_GROUPS=<n> caps the group count (experiments).
 template <class B, int NTH, class SmemFn>
 int tc_geometry_of(int device, SmemFn smem_bytes, long batch, Geom& g) {
@@ -752,12 +749,10 @@ int tc_geometry_of(int device, SmemFn smem_bytes, long batch, Geom& g) {
   for (int groups = 4; groups >= 1; groups--) {
     const int nthr = groups * TC_M;
     if (nthr > BodyMaxThreads<B>::v || (want_groups && groups > want_groups)) continue;
-    if (groups > tc_tmem_slots(NTH) && tc_tmem_slots(NTH) < 2) continue;          // sharing needs at least two slots
     size_t smem = smem_bytes(nthr);
     if (smem + 128 > max_smem) continue;
     int occ = rt_occupancy<B>(nthr, smem);
     if (occ <= 0) continue;
-    occ = std::min(occ, std::max(1, 512 / tc_tmem_cols<NTH>(groups)));            // TMEM columns of the SM
     const long slots = (long)rt_sm_count(device) * occ;
     int use = groups;
     // less than one wave of rows (a small batch, or the tail the callers split off): the fewest groups per CTA that still
@@ -1114,9 +1109,9 @@ int do_priv_setup(pai_priv* k, rt_stream s) {
 // ================================================================================================ C ABI
 // ---- warp-per-ciphertext path (pai_coop.cuh) -------------------------------------------------------------------
 // A batch, or the tail of a batch beyond whole waves of the throughput kernel, of at most coop_limit(wave) elements
-// takes it.  Measured at 2048-bit keys (profiles/README.md): a wave of the thread-per-ciphertext kernel costs the same
-// 220 ms (encrypt) / 69 ms (decrypt) whether it holds 1 or 33 152 ciphertexts, the warp kernels run at ~0.35x of its
-// full-wave throughput with a 20 ms / 4 ms floor -- so they win up to about a third of a wave.
+// takes it.  A wave of the thread-per-ciphertext kernel costs the same whether it holds one ciphertext or a full wave,
+// while the warp kernels run at a fraction of its full-wave throughput with a small floor -- so they win up to about a
+// third of a wave.
 // PAI_COOP_MAX overrides the limit with an absolute element count (0 disables the path).
 static long coop_limit(long wave) {
   const char* e = getenv("PAI_COOP_MAX");
@@ -1385,7 +1380,7 @@ int pai_pub_create(const uint32_t* n, int limbs, int device, pai_pub** out) {
   // the operand buffers of even one 128-thread group no longer fit shared memory)
   if (!rc && tc_supported(2 * ntp, 12)) {
     DISPATCH_TC(2 * ntp, rc = do_tc_setup<NTH>(k, 0));
-    k->use_tc = !rc && k->use_digit && tc_wanted(2 * ntp, 4);
+    k->use_tc = !rc && k->use_digit && tc_wanted();
     const char* st = getenv("PAI_TC_STAGGER");
     k->tc_stagger = st && *st ? atoi(st) : 40000;
   }
@@ -1632,7 +1627,7 @@ int pai_priv_create(const uint32_t* p, const uint32_t* q, int limbs, int device,
   { const char* e = getenv("PAI_DECRYPT_PATH"); k->use_digit = !(e && std::string(e) == "full"); }
   if (!rc && tc_supported(ntp, 8)) {            // tensor-core reductions: p, q of 64 .. 256 base-256 digits (keys up to 4096 bits)
     DISPATCH_TC(ntp, rc = do_priv_tc_setup<NTH>(k, 0));
-    k->use_tc = !rc && k->use_digit && tc_wanted(ntp, 2);
+    k->use_tc = !rc && k->use_digit && tc_wanted();
     const char* st = getenv("PAI_TC_STAGGER");
     k->tc_stagger = st && *st ? atoi(st) : 40000;
   }

@@ -3,7 +3,7 @@
 // Each program is the work ONE thread does for ONE batch element.  The __global__ wrappers in
 // pai_engine.cu run them in a persistent grid (thousands of elements per launch); tests/hostsim
 // runs the same programs on the CPU (test-only).  Reference semantics, file:line in
-// /root/reference (data61/python-paillier):
+// data61/python-paillier 1.5.0:
 //   prog_encrypt   PaillierPublicKey.raw_encrypt          phe/paillier.py:102-139
 //   prog_decrypt   PaillierPrivateKey.raw_decrypt + crt   phe/paillier.py:328-374
 //   prog_mulmod    EncryptedNumber._raw_add / util.mulmod phe/paillier.py:705-719, phe/util.py:53-64

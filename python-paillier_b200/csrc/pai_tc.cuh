@@ -1,13 +1,14 @@
-// pai_tc.cuh -- digit Montgomery arithmetic modulo n^2 with the REDUCTIONS on the 5th-generation tensor cores.
+// pai_tc.cuh -- digit Montgomery arithmetic modulo n^2 with the REDUCTIONS on the tensor cores (Hopper wgmma).
 //
 // Every Montgomery reduction multiplies a per-ciphertext number by a batch-wide constant twice:
 //     m = T_lo * N' mod R        (N' = -n^-1 mod R)          and          hi = floor(m * n / R).
-// In base-256 digits, for the 128 ciphertexts of a thread group at once, that is  [128 x D] x Toeplitz(const):
-// one tcgen05.mma kind::i8 GEMM each (M = 128 TMEM lanes = 128 ciphertexts, N = D digit columns, K = D digits, u8 x u8
-// -> s32 column sums <= D * 255^2 < 2^24).  The thread that owns row i reads its column sums back with tcgen05.ld,
-// propagates the carries (ALU pipe) and has the quotient / the high half as ordinary 32-bit limbs again.  What stays on
-// the integer-multiply pipe are only the products of two per-ciphertext numbers (x0*y0, x0*y1 + x1*y0): 100 instead
-// of 228 tile products per squaring, 192 instead of 320 per multiplication at 2048-bit keys, and no quotient products.
+// In base-256 digits, for the 128 ciphertexts of a thread group (one warpgroup) at once, that is  [128 x D] x Toeplitz(const):
+// wgmma.mma_async u8 x u8 -> s32 GEMMs (two m64 halves of the 128 rows, K = 32 digits per instruction, column sums
+// <= D * 255^2 < 2^24).  The accumulator fragments are computed 32 columns at a time and moved by warp shuffles to the
+// lane that owns the row, which propagates the carries (ALU pipe) and has the quotient / the high half as ordinary 32-bit
+// limbs again.  What stays on the integer-multiply pipe are only the products of two per-ciphertext numbers (x0*y0,
+// x0*y1 + x1*y0): 100 instead of 228 tile products per squaring, 192 instead of 320 per multiplication at 2048-bit keys,
+// and no quotient products.
 //
 // Exactness of the high half.  GEMM 2 produces the byte columns D-4 .. 2D-5 of m*n (the top three columns 2D-4 .. 2D-2
 // are six scalar byte products).  The columns below D-4 are never computed: their sum I is < 1.004 * 256^(D-2), and the
@@ -24,11 +25,13 @@
 //   G2  A x Toeplitz(n)               E4: z = B_hi + hi' + ... (< 3n + 3) -> Z1 in place, reduced by digit_reduce3
 //   Z0 = t - n*carry: park -> the buffer of x1.       Shared memory per ciphertext: 3 half-buffers (x0, x1, A).
 //
-// A CTA runs two independent groups of 128 threads (named barriers, own mbarrier, own 256 TMEM columns): while one
-// group waits for its GEMMs and runs the ALU epilogues, the other one keeps the integer-multiply pipe busy.
+// A CTA runs up to four independent groups of 128 threads (named barriers): while one group waits for its GEMMs and runs
+// the ALU epilogues, the others keep the integer-multiply pipe busy.  PTX does not promise which rows of A a warp's share
+// of a wgmma reads, so after every GEMM chunk the four warps of the group meet at their named barrier before any of them
+// rewrites A (tc_ld32).
 //
-// Compiled twice like everything else: nvcc (sm_100a: tcgen05 / TMEM / mbarrier inline PTX) and g++ -DPAI_HOSTSIM, where
-// a "group" is 8 rows walked phase by phase and the GEMM is an integer loop over the very same operand layouts.
+// Compiled twice like everything else: nvcc (sm_90a: wgmma inline PTX) and g++ -DPAI_HOSTSIM, where a "group" is TC_RL
+// rows walked phase by phase and the GEMM is an integer loop over the very same operand layouts.
 #pragma once
 #include "pai_digit.cuh"
 
@@ -40,7 +43,7 @@ constexpr int TC_RL = 2;                  // rows of a group the simulation walk
 constexpr int TC_RL = 1;                  // the GPU thread owns one row; state lives in registers
 #endif
 #define TC_EACH_ROW for (int rw = 0; rw < TC_RL; rw++)
-constexpr int TC_M = 128;                 // rows (ciphertexts) of a group = TMEM lanes
+constexpr int TC_M = 128;                 // rows (ciphertexts) of a group = the M of two m64 wgmma halves
 
 // ---- operand layouts (K-major, no swizzle: 8 x 16-byte core matrices) ---------------------------------------------
 // A operand [128 x D]: digit k of row r.  Core matrix (r/8, k/16) at ((r/8) * (D/16) + k/16) * 128 bytes.
@@ -96,14 +99,7 @@ struct TcCtx {
 #if defined(PAI_HOSTSIM)
   int32_t tmem[TC_RL][512];
 #else
-  uint32_t tmem;            // TMEM address of the accumulator this group currently uses (lane 0, first column)
-  uint32_t tmem_base;       // first column of the CTA's TMEM allocation
-  int nslots;               // accumulator slots of D columns in it; groups > nslots: slots are taken per reduction
-  uint32_t* locks;          // shared: one word per slot (0 free / 1 taken) followed by one slot-index word per group
-  int slot;                 // slot held (static assignment: the group index)
-  int ngroups;
-  uint64_t* mbar;           // the group's mbarrier
-  uint32_t phase;
+  int which;                // operand band of the current reduction GEMM: 0 = N', 1 = n (see tc_ld32)
   int grp;                  // group index (named barrier 1 + grp)
   long long* prof;          // optional phase profile (PAI_TC_PROF): 16 cycle counters per warp, or null
 #endif
@@ -170,31 +166,25 @@ PAI_DEV uint64_t tc_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
   d |= (uint64_t)((saddr >> 4) & 0x3fff);
   d |= (uint64_t)((lbo >> 4) & 0x3fff) << 16;
   d |= (uint64_t)((sbo >> 4) & 0x3fff) << 32;
-  d |= (uint64_t)1 << 46;                                 // descriptor version of sm_100
   return d;
 }
-// instruction descriptor: D = s32, A = B = unsigned 8 bit, both K-major, dense
-PAI_DEV uint32_t tc_idesc(int n, int m) { return (2u << 4) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24); }
-PAI_DEV void tc_mma(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
+// d[64 x 32] (+)= A[64 x 32 digits] x B[32 digits x 32], unsigned 8-bit operands, s32 accumulators
+PAI_DEV void tc_wgmma_n32(uint32_t d[16], uint64_t da, uint64_t db, uint32_t accumulate) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k32.s32.u8.u8 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p;\n\t}\n"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]),
+        "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+      : "l"(da), "l"(db), "r"(accumulate)
       : "memory");
-}
-PAI_DEV void tc_mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(tc_smem_u32(bar)), "r"(count));
-}
-PAI_DEV void tc_mbar_wait(uint64_t* bar, uint32_t phase) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tTC_WAIT:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra TC_DONE;\n\tbra TC_WAIT;\n\tTC_DONE:\n\t}\n" ::"r"(tc_smem_u32(bar)), "r"(phase)
-      : "memory");
-}
-PAI_DEV void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(tc_smem_u32(bar)) : "memory");
 }
 PAI_DEV void tc_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
+// x[i] for a lane-dependent i in 0..3 without indexing registers (which would put x in local memory)
+PAI_DEV uint32_t tc_pick4(const uint32_t x0, const uint32_t x1, const uint32_t x2, const uint32_t x3, int i) {
+  const uint32_t lo = (i & 1) ? x1 : x0, hi = (i & 1) ? x3 : x2;
+  return (i & 2) ? hi : lo;
+}
 #endif
 
 // 32 consecutive column sums of this thread's row, starting at column c0
@@ -203,26 +193,64 @@ PAI_DEV void tc_ld32(const TcCtx<NTH>& c, int rw, int c0, uint32_t v[32]) {
 #if defined(PAI_HOSTSIM)
   for (int j = 0; j < 32; j++) v[j] = (uint32_t)c.tmem[rw][c0 + j];
 #else
+  // The columns c0 .. c0 + 31 of the GEMM c.which, computed now: both m64 halves, over the K blocks that reach them (both
+  // Toeplitz operands are triangular: digit block kappa of A reaches only the columns j >= 32 kappa of A x T(N') and
+  // only the columns j' < 32 kappa + 48 of A x T(n)).
   (void)rw;
-  const uint32_t taddr = c.tmem + (((uint32_t)(c.row0 & ~31)) << 16) + (uint32_t)c0;      // lane quarter of this warp
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-        "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),
-        "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-        "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+  const int D = 32 * NTH, t = c0 >> 5;
+  uint32_t acc[2][16];
+  PAI_UNROLL
+  for (int h = 0; h < 2; h++) {
+    PAI_UNROLL
+    for (int i = 0; i < 16; i++) acc[h][i] = 0;
+  }
+  asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+  const uint32_t a0 = tc_smem_u32(c.A), b0 = tc_smem_u32(c.band[c.which]);
+  uint32_t more = 0;
+  PAI_UNROLL
+  for (int kap = 0; kap < NTH; kap++) {
+    if (c.which == 0 ? kap > t : kap < t - 1) continue;
+    const uint64_t db = tc_desc(b0 + (uint32_t)((D - 32 - 32 * kap + c0) / 8) * 256u, 128u, 256u);
+    PAI_UNROLL
+    for (int h = 0; h < 2; h++)
+      tc_wgmma_n32(acc[h], tc_desc(a0 + (uint32_t)(h * 64 * D + kap * 256), 128u, (uint32_t)(D / 16) * 128u), db, more);
+    more = 1;
+  }
+  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+  asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+  tc_bar_sync(1 + c.grp, TC_M);            // every warp's chunk is complete before any warp rewrites A (E1, E2, P2)
+  // Fragment of lane L = 4 g + q: in 8-column block j, acc[h][4j + 2k' + e] = (row g + 8k' of the warp's 16 in half h,
+  // column 8j + 2q + e).  Lane L owns the warp's row (L & 15) of half (L >> 4), i.e. local row g' + 8k with g' = L & 7,
+  // k = L >> 3 (c.row0).  In round r it takes the column pair 2q' + (0, 1), q' = (r + k) & 3, from lane 4g' + q' -- which
+  // sends, in that round, its pair of local row g' + 8((q' - r) & 3).
+  const int lane = threadIdx.x & 31, qs = lane & 3, gd = lane & 7, kd = lane >> 3;
+  PAI_UNROLL
+  for (int j = 0; j < 4; j++) {
+    uint32_t got[4][2];
+    PAI_UNROLL
+    for (int r = 0; r < 4; r++) {
+      const int ks = (qs - r) & 3, src = 4 * gd + ((r + kd) & 3);
+      PAI_UNROLL
+      for (int e = 0; e < 2; e++) {
+        const uint32_t s = tc_pick4(acc[0][4 * j + e], acc[0][4 * j + 2 + e], acc[1][4 * j + e], acc[1][4 * j + 2 + e], ks);
+        got[r][e] = __shfl_sync(0xffffffffu, s, src);
+      }
+    }
+    PAI_UNROLL
+    for (int q = 0; q < 4; q++) {
+      const int r = (q - kd) & 3;
+      PAI_UNROLL
+      for (int e = 0; e < 2; e++) v[8 * j + 2 * q + e] = tc_pick4(got[0][e], got[1][e], got[2][e], got[3][e], r);
+    }
+  }
 #endif
 }
 
 // The group's GEMM: accumulator = A x window(band[which]).  All threads of the group call it.
 template <int NTH>
 PAI_DEV void tc_gemm(TcCtx<NTH>& c, int which) {
-  const int D = 32 * NTH;
 #if defined(PAI_HOSTSIM)
+  const int D = 32 * NTH;
   const uint8_t* a = (const uint8_t*)c.A;
   TC_EACH_ROW {
     const int r = c.row0 + rw;
@@ -242,67 +270,11 @@ PAI_DEV void tc_gemm(TcCtx<NTH>& c, int which) {
     }
   }
 #else
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");        // generic-proxy writes of A -> tensor-core reads
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");    // our tcgen05.ld of the previous accumulator are done
-  if (which == 0 && c.ngroups > c.nslots) {
-    // more groups than accumulator slots (three groups, two 256-column slots at 2048-bit keys): a group holds a slot
-    // from the first GEMM of a reduction to the end of its second epilogue -- about a third of its time
-    if (c.row0 == 0) {
-      int sl = c.grp % c.nslots;
-      while (atomicCAS(&c.locks[sl], 0u, 1u) != 0u) { sl = sl + 1 == c.nslots ? 0 : sl + 1; __nanosleep(100); }
-      __threadfence_block();
-      c.locks[4 + c.grp] = (uint32_t)sl;
-    }
-  }
+  // the GEMM itself runs chunk by chunk as the epilogue reads it (tc_ld32); here the rows of A written through the generic
+  // proxy are made visible to the tensor cores
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   tc_bar_sync(1 + c.grp, TC_M);
-  if (which == 0 && c.ngroups > c.nslots) {
-    c.slot = (int)((volatile uint32_t*)c.locks)[4 + c.grp];
-    c.tmem = c.tmem_base + (uint32_t)(c.slot * D);
-  }
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  if (c.row0 == 0) {
-    // Both Toeplitz operands are triangular: digit block kappa of A reaches only the columns j >= 32 kappa of A x T(N')
-    // (N'[j - k] = 0 for j < k) and only the columns j' < 32 kappa + 35 of A x T(n) (n[D - 4 + j' - k] = 0 beyond k + 3).
-    // Each K step therefore issues its MMA over that column range only (a multiple of 16), widest step first so that it
-    // initialises every column; about half of the tensor work of a full D x D product.  One MMA covers at most 256
-    // columns: wider moduli (D = 384 at 3072-bit keys) take two column blocks per K step.
-    const uint32_t a0 = tc_smem_u32(c.A), b0 = tc_smem_u32(c.band[which]);
-    bool first = true;
-#pragma unroll
-    for (int step = 0; step < NTH; step++) {
-      const int kap = which == 0 ? step : NTH - 1 - step;
-      const int c_lo = which == 0 ? 32 * kap : 0;
-      const int c_hi = which == 0 ? D : (32 * kap + 48 < D ? 32 * kap + 48 : D);
-      const uint64_t da = tc_desc(a0 + (uint32_t)kap * 2u * 128u, 128u, (uint32_t)(D / 16) * 128u);
-#pragma unroll
-      for (int n0 = 0; n0 < D; n0 += 256) {
-        const int lo = c_lo > n0 ? c_lo : n0;
-        const int hi = c_hi < n0 + 256 ? c_hi : n0 + 256;
-        if (lo >= hi) continue;
-        const uint64_t db = tc_desc(b0 + (uint32_t)((D - 32 - 32 * kap + lo) / 8) * 256u, 128u, 256u);
-        tc_mma(c.tmem + (uint32_t)lo, da, db, tc_idesc(hi - lo, TC_M), first ? 0u : 1u);
-      }
-      first = false;
-    }
-    tc_commit(c.mbar);
-  }
-  tc_mbar_wait(c.mbar, c.phase);
-  c.phase ^= 1u;
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#endif
-}
-
-// end of a reduction: the group is done reading its accumulator; with more groups than slots the slot is handed back
-template <int NTH>
-PAI_DEV void tc_tmem_release(TcCtx<NTH>& c) {
-#if !defined(PAI_HOSTSIM)
-  if (c.ngroups > c.nslots) {
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    tc_bar_sync(1 + c.grp, TC_M);
-    if (c.row0 == 0) { __threadfence_block(); atomicExch(&c.locks[c.slot], 0u); }
-  }
-#else
-  (void)c;
+  c.which = which;
 #endif
 }
 
@@ -459,15 +431,28 @@ PAI_FN void tc_prod1_sqr(SOpnd A, Opnd P, SOpnd x0, TcRow* st) {
   }
 }
 
-// E1: quotient m = (column sums of lo * N') mod R -> A (as limbs == digits)
+// E1: quotient m = (column sums of lo * N') mod R -> A (as limbs == digits).  Column block t of the product depends on the
+// digit blocks 0 .. t of A only, so the blocks are read from the top down and each one's limbs, without the carry from
+// below, replace digit block t as soon as no lower block needs it; a second pass adds the carries.
 template <int NTH>
 PAI_FN void tc_epi_m(const TcCtx<NTH>* c, int rw, SOpnd A) {
-  uint32_t carry = 0;
-  for (int t = 0; t < NTH; t++) {
+  uint32_t ovf[NTH];
+  PAI_UNROLL
+  for (int t = NTH - 1; t >= 0; t--) {
     uint32_t v[32], l[8];
+    ovf[t] = 0;
     tc_ld32<NTH>(*c, rw, 32 * t, v);
-    tc_limbs8(v, carry, l);
+    tc_limbs8(v, ovf[t], l);
     st_tile(A, t, l);
+  }
+  uint32_t carry = 0;
+  PAI_UNROLL
+  for (int t = 0; t < NTH; t++) {
+    uint32_t l[8], r[8];
+    ld_tile(A, t, l);
+    const uint32_t cy = add8_small(r, l, carry);
+    st_tile(A, t, r);
+    carry = ovf[t] + cy;
   }
 }
 
@@ -513,7 +498,7 @@ PAI_FN void tc_epi_t(const TcCtx<NTH>* c, int rw, SOpnd A, Opnd Ag, Opnd P, Opnd
   constexpr int BL = NTH > 8 ? NTH / 2 : NTH;                   // park tiles loaded together (register budget)
   uint32_t th[BL][8];
   PAI_UNROLL
-  for (int j = 0; j < BL; j++) ld_tile(P, j, th[j]);             // park loads in flight before the first TMEM read
+  for (int j = 0; j < BL; j++) ld_tile(P, j, th[j]);             // park loads in flight before the first GEMM chunk
   TcHi<NTH> h;
   tc_hi_begin<NTH>(*c, rw, st->ltop, h);
   uint32_t cy = h.cadd, bo = 0;
@@ -788,7 +773,6 @@ PAI_DEV void tc_op(TcCtx<NTH>& c, FX0 x0, FX1 x1, FY0 y0, FY1 y1) {
   TC_PROF(c, t0, 3);
   constexpr bool SWAP = SQR && tc_x1_global<NTH>();      // squarings with x1 in global memory stage it in A (tc_prod2_sqr_g)
   TC_EACH_ROW tc_epi_t<NTH, SWAP>(&c, rw, tc_as<NTH>(c, rw), tc_a<NTH>(c, rw), tc_park<NTH>(c, rw), tc_wslot<NTH>(c, rw), c.dc, &st[rw]);
-  tc_tmem_release<NTH>(c);
   TC_PROF(c, t0, 4);
   TC_EACH_ROW {
     if constexpr (SWAP) tc_prod2_sqr_g<NTH>(tc_as<NTH>(c, rw), tc_wslot<NTH>(c, rw), tc_xs<NTH>(c, rw), x0(rw), x1(rw), &st[rw]);
@@ -803,7 +787,6 @@ PAI_DEV void tc_op(TcCtx<NTH>& c, FX0 x0, FX1 x1, FY0 y0, FY1 y1) {
   tc_gemm<NTH>(c, 1);
   TC_PROF(c, t0, 3);
   TC_EACH_ROW tc_epi_z<NTH>(&c, rw, tc_as<NTH>(c, rw), tc_xs<NTH>(c, rw), tc_h<NTH>(c, 0, rw), c.dc, &st[rw]);
-  tc_tmem_release<NTH>(c);
   TC_PROF(c, t0, 6);
   TC_EACH_ROW {
     big_copy<NTH>(tc_h<NTH>(c, 1, rw), tc_h<NTH>(c, 0, rw));                                     // Z1 -> buffer 1

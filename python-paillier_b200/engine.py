@@ -179,7 +179,7 @@ class Engine:
         path = lib_path or os.path.join(_HERE, LIB_NAME)
         if not os.path.exists(path):
             raise EngineUnavailable(
-                "%s not found: build it with `python __graft_entry__.py` (nvcc, sm_100a). "
+                "%s not found: build it with `python __graft_entry__.py` (nvcc, sm_90a). "
                 "This package has no CPU fallback." % path)
         try:
             self.lib = ctypes.CDLL(path)

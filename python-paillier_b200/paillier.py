@@ -1,7 +1,7 @@
-"""Drop-in ``phe.paillier`` API on top of the B200 engine.
+"""Drop-in ``phe.paillier`` API on top of the H100 engine.
 
 Same classes, method names, argument meaning and exceptions as the reference
-(/root/reference/phe/paillier.py); the big-integer work -- ``r^n mod n^2`` (:137, :622), the CRT pair
+(phe/paillier.py of data61/python-paillier 1.5.0); the big-integer work -- ``r^n mod n^2`` (:137, :622), the CRT pair
 (:346-353), ``a*b mod n^2`` (:719), ``c^k mod n^2`` (:749-751) -- runs in the CUDA kernels, batch of
 one for the scalar methods and full batches for the ``*_batch`` methods / ``EncryptedVector``
 (vector.py).  Nothing here falls back to CPU bigint arithmetic for those operations.

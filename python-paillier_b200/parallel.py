@@ -1,6 +1,6 @@
 """Multi-GPU plumbing: one process per GPU (torchrun), batches shard by contiguous row ranges.
 
-The hot path has no exchange step -- every element is independent (SURVEY.md section 8e) -- so the only
+The hot path has no exchange step -- every element is independent -- so the only
 collectives are (1) a broadcast of the key limbs from rank 0 and (2) an optional all-gather of result
 limbs when a caller wants the whole vector on every rank.  NCCL on GPUs, gloo in the CPU tests.
 """

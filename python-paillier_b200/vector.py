@@ -96,7 +96,7 @@ def random_r_values(n, count):
 
 
 # ------------------------------------------------------------------------------------------------------
-# Vectorised EncodedNumber.encode / decode (SURVEY.md section 8f, rank 1): numpy fast paths that give exactly
+# Vectorised EncodedNumber.encode / decode: numpy fast paths that give exactly
 # the values phe/encoding.py:110-233 computes element by element, with a per-element fallback for
 # everything outside the fast path (huge mantissas, precision=..., non-finite values, ints beyond 63 bits).
 def _limbs_from_signed(int_rep, n, ln):

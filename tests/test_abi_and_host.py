@@ -113,7 +113,7 @@ int main() { row<2>(); row<4>(); row<6>(); row<8>(); row<12>(); return 0; }
     exe = tmp_path / "budget"
     subprocess.run(["g++", "-std=c++17", "-x", "c++", str(src), "-o", str(exe)], check=True)
     out = subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout.split("\n")
-    limit = 232448 - 128                                   # cudaDevAttrMaxSharedMemoryPerBlockOptin on sm_100 minus the margin
+    limit = 232448 - 128                                   # cudaDevAttrMaxSharedMemoryPerBlockOptin on sm_90 minus the margin
     fits = {}
     for line in out:
         if line.strip():

@@ -198,7 +198,7 @@ def test_streams_and_cuda_graph(pkg, cuda_engine, gmp):
 
 
 def test_all_kernel_paths_agree(pkg, cuda_engine, monkeypatch):
-    """The tensor-core reduction kernels (default, pai_tc.cuh), the base-n digit kernels on the integer pipe (PAI_TC=0),
+    """The tensor-core reduction kernels (PAI_TC=2, pai_tc.cuh), the base-n digit kernels on the integer pipe (default),
     the full-width Montgomery kernels (PAI_*_PATH=full) and the warp-per-ciphertext kernels (small batches, pai_coop.cuh)
     must give identical bits."""
     n, p, q = _key(1024)

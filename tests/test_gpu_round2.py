@@ -158,8 +158,8 @@ def test_vector_inside_a_torch_stream(pkg, cuda_engine):
 
 
 def test_fused_reductions_on_gpu(pkg, cuda_engine):
-    """EncryptedVector.sum / dot on the GPU (shared-memory product tree, second launch over the CTA partials, Straus groups
-    on the tensor-core kernels) against the launch chains of round 1 and the plaintext results."""
+    """EncryptedVector.sum / dot on the GPU (shared-memory product tree, second launch over the CTA partials; the dot
+    product's powers on the default digit kernels) against the launch chains and the plaintext results."""
     import torch
     n, p, q = _key(1024)
     pk = pkg.PaillierPublicKey(n)

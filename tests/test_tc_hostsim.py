@@ -1,5 +1,5 @@
 """The tensor-core kernel family (pai_tc.cuh) on the test-only host simulation, where a thread group is walked phase by
-phase and the tcgen05 GEMM is an integer loop over the very same operand / band layouts: encrypt, CRT decrypt and
+phase and the wgmma GEMM is an integer loop over the very same operand / band layouts: encrypt, CRT decrypt and
 raw_mul must equal the oracle and the integer-pipe digit kernels (PAI_TC=0) bit for bit, for every key size the family
 covers, including degenerate ciphertexts and batches that are not a multiple of the group."""
 import random
@@ -50,14 +50,21 @@ def test_tc_family_equals_oracle_and_digit_family(pkg, sim, monkeypatch, kb, row
 
 
 def test_tc_family_key_size_coverage(pkg, sim, monkeypatch):
-    """Which keys take the tensor-core kernels by default: encrypt for 1024 .. 3072-bit keys, decrypt for 1024 .. 4096-bit
-    keys; smaller or odd-sized ones stay on the integer-pipe digit kernels (same bits either way,
-    tests/test_edge_keys_hostsim.py).  PAI_TC=2 forces the family wherever it is instantiated (used by the other test)."""
-    monkeypatch.delenv("PAI_TC", raising=False)
+    """Which keys the tensor-core kernels cover under PAI_TC=2: encrypt for 1024 .. 3072-bit keys, decrypt for 1024 .. 4096-bit
+    keys (same bits as the integer-pipe digit kernels, tests/test_edge_keys_hostsim.py).  By default every key, 256 to
+    4096 bits, takes the integer-pipe digit kernels."""
     for kb, enc, dec in ((256, "digit", "digit"), (512, "digit", "digit"), (1024, "tc", "tc"), (2048, "tc", "tc"), (3072, "tc", "tc"),
                          (4096, "digit", "tc")):
         fx = load_golden("vectors_%d.json" % kb)
-        pub = pkg.PublicContext(H(fx["n"]), engine=sim)
-        priv = pkg.PrivateContext(H(fx["p"]), H(fx["q"]), engine=sim)
-        assert (pub.kernel_path(), priv.kernel_path()) == (enc, dec), kb
-        pub.close(); priv.close()
+        for forced in (True, False):
+            if forced:
+                monkeypatch.setenv("PAI_TC", "2")
+            else:
+                monkeypatch.delenv("PAI_TC", raising=False)
+            pub = pkg.PublicContext(H(fx["n"]), engine=sim)
+            priv = pkg.PrivateContext(H(fx["p"]), H(fx["q"]), engine=sim)
+            if forced and kb >= 1024:
+                assert (pub.kernel_path(), priv.kernel_path()) == (enc, dec), kb
+            elif not forced:
+                assert (pub.kernel_path(), priv.kernel_path()) == ("digit", "digit"), kb
+            pub.close(); priv.close()

@@ -1,4 +1,4 @@
-"""EncryptedVector and the vectorised EncodedNumber encode/decode (SURVEY.md 8f rank 1) on the test-only
+"""EncryptedVector and the vectorised EncodedNumber encode/decode on the test-only
 host simulation: results must equal the per-element reference semantics exactly."""
 import importlib
 import random
