@@ -120,6 +120,26 @@ int pai_raw_sum(pai_pub* k, const uint32_t* d_c, long batch, uint32_t* d_out, vo
  * (examples/logistic_regression_encrypted_model.py:170-180, phe/tests/math_test.py:50-58).  batch >= 1. */
 int pai_raw_dot(pai_pub* k, const uint32_t* d_a, const uint32_t* d_s, uint32_t* d_out, int32_t* d_status, long batch, void* stream);
 
+/* out[j] = prod_{t = indptr[j]}^{indptr[j+1]-1} ( neg[t] ? c[indices[t]]^-1 : c[indices[t]] ) ^ mag[t]  mod n^2
+ * A plaintext matrix in CSR form times a ciphertext vector: the encrypted scoring loop of
+ * examples/logistic_regression_encrypted_model.py:170-180 (score += x[0, i] * weights[i] over the nonzeros of a row) for
+ * every row at once.  c: [ncols][pai_pub_c_limbs()].  indptr: [nrows + 1] int64; indices: [nnz] int32 column numbers in
+ * [0, ncols).  mag: [nnz][mag_limbs] magnitudes, 0 <= mag < n.  mag_bits: a bound on the bit length of every magnitude
+ * (0 = 32 * mag_limbs); it only steers the choice of the window width (a 0/1 matrix passes 1).
+ * Scalars are sign and magnitude, not residues as in pai_raw_mul's s: the reference's rule for an encoding s
+ * (phe/paillier.py:742-749: s >= n - max_int -> base invert(c, n^2), exponent n - s) becomes neg = 1, mag = n - s; any
+ * other s is neg = 0, mag = s.  neg: [nnz] uint8, or NULL when every scalar is non-negative.
+ * status: [ncols] (may be NULL), 1 where c[i] is used with a negative scalar and has no inverse mod n^2 (the outputs of
+ * the rows that use it are then unspecified), else 0.  Rows with no entries give 1.
+ * Window tables c^1 .. c^(2^w - 1) are built once per column (and per inverse) and shared by all rows; every row runs
+ * one squaring chain for all its entries (Straus).  w comes from pai_raw_matvec_window.  One thread per row: a 1 x d
+ * product is latency bound, pai_raw_dot is the tool for it.  Asynchronous on `stream`; no host synchronisation. */
+int pai_raw_matvec(pai_pub* k, const uint32_t* d_c, long ncols, const int64_t* d_indptr, const int32_t* d_indices,
+                   const uint32_t* d_mag, int mag_limbs, int mag_bits, const uint8_t* d_neg, long nnz, long nrows,
+                   uint32_t* d_out, int32_t* d_status, void* stream);
+/* the window width 1..8 pai_raw_matvec picks for these shapes (bits = mag_bits, or 32 * mag_limbs; with_neg: d_neg given) */
+int pai_raw_matvec_window(pai_pub* k, long ncols, long nrows, long nnz, int bits, int with_neg);
+
 /* ---- private key: PaillierPrivateKey (phe/paillier.py:197-380) ---------------------------------
  * p, q: `limbs` limbs each, p*q = n.  Ordered internally so that p < q (:224-229).  All derived
  * constants (p^2, q^2, p^-1 mod q, hp, hq; :230-235) are computed by the engine on the device. */

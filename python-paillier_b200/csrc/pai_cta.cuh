@@ -701,4 +701,58 @@ PAI_DEV void cta_powmod_digit(u4* smem, const CtaId& id, const uint32_t* base, c
   }
 }
 
+// ---- plaintext CSR matrix times ciphertext vector in digit form (pai_raw_matvec).  consts = dc_pow_limbs, two buffers.
+// Tables: one thread per slot (see prog_matvec_table); slot ncols + i is built from cinv[i] only where flag[i] is set.
+template <int NTH>
+PAI_DEV void cta_matvec_table(u4* smem, const CtaId& id, const uint32_t* c, const uint32_t* cinv, const int32_t* flag,
+                              long ncols, long nslots, int w, u4* tbl, const uint32_t* gzero) {
+  DigitEnv dc;
+  digit_bind_pow<NTH>(dc, smem, gzero);
+  DPowEnv<NTH> E;
+  cta_bufs<2 * NTH>(E.buf, 2, smem, dc_pow_limbs(NTH) / 4, id);
+  E.tbl = E.buf[0];                                         // (the shared tables are addressed by mv_entry)
+  E.dc = &dc;
+  E.step_sync = 0;
+  const int lc = 16 * NTH;
+  for (long s = (long)id.cta * id.nthr + id.tid; s < nslots; s += (long)id.ncta * id.nthr) {
+    const bool inv = s >= ncols;
+    const long col = inv ? s - ncols : s;
+    if (inv && !flag[col]) continue;
+    prog_matvec_table<NTH>(E, (inv ? cinv : c) + col * lc, tbl, s, w);
+  }
+}
+
+// Rows: one thread per output row, handed out by the row scheduler.  The window count comes from the largest magnitude
+// of the row, made warp-uniform, so the lanes of a warp run the same squaring chain.  Rows beyond the last one repeat it
+// without storing (the warp stays complete for the reduction).
+template <int NTH>
+PAI_DEV void cta_matvec_digit(u4* smem, const CtaId& id, const u4* tbl, long ncols, int w, const int64_t* indptr,
+                              const int32_t* indices, const uint32_t* mag, int ml, const uint8_t* neg, uint32_t* out,
+                              long nrows, unsigned long long* counter, const uint32_t* gzero) {
+  DigitEnv dc;
+  digit_bind_pow<NTH>(dc, smem, gzero);
+  DPowEnv<NTH> E;
+  cta_bufs<2 * NTH>(E.buf, 2, smem, dc_pow_limbs(NTH) / 4, id);
+  E.tbl = E.buf[0];
+  E.dc = &dc;
+  E.step_sync = 0;
+  const int lc = 16 * NTH;
+  RowSched sched = sched_init(id, counter, nrows);
+  for (long g = sched_next_row(sched, id); g >= 0; g = sched_next_row(sched, id)) {
+    bool store = g < nrows;
+    if (!store) g = nrows - 1;
+    const long lo = indptr[g], hi = indptr[g + 1];
+    int nbits = 0;
+    for (long t = lo; t < hi; t++) {
+      const int b = limbs_bitlen(mag + t * ml, ml);
+      nbits = b > nbits ? b : nbits;
+    }
+    int nwin = (nbits + w - 1) / w;
+#if !defined(PAI_HOSTSIM)
+    nwin = __reduce_max_sync(0xffffffffu, nwin);
+#endif
+    prog_matvec_row<NTH>(E, tbl, ncols, w, nwin, indices, mag, ml, neg, lo, hi, out + g * lc, store);
+  }
+}
+
 }  // namespace pai

@@ -723,23 +723,100 @@ PAI_DEV void prog_decrypt_digit(DPowEnv<NTP>& E, DSideC<NTP>& P, DSideC<NTP>& Qs
 
 
 // ------------------------------------------------------------------------------------------------
-// c^k mod n^2 with per-element exponents in digit form (EncryptedNumber._raw_mul, phe/paillier.py:749-751).
-//   base row: plain ciphertext, 2*NTH tiles = c_0 + c_1*R;  e: exponent limbs of this element; nwin uniform.
-template <int NTH, int W>
-PAI_DEV void prog_powmod_digit(DPowEnv<NTH>& E, const uint32_t* base_row, const uint32_t* e, int nl, int nwin,
-                               uint32_t* out_row, bool store) {
+// Entering and leaving the digit-Montgomery domain of n^2 for a plain ciphertext row (2*NTH tiles = c_0 + c_1*R).
+// Entry: c*R = dmul((c_0, 0), RR) + dmul((c_1, 0), E3), left in buf[0] as [d1 | d0] (swapped = 1); uses both buffers.
+template <int NTH>
+PAI_DEV void digit_enter(const DPowEnv<NTH>& E, const uint32_t* base_row) {
   const DigitEnv& dc = *E.dc;
   Opnd c0{(u4*)base_row, 1}, c1{(u4*)(base_row + 8 * NTH), 1};
   dmul<NTH>(half_lo<NTH>(E.buf[0]), half_hi<NTH>(E.buf[0]), c0, dc.ZERO, dc.RR.d0, dc.RR.d1, &dc);
   dmul<NTH>(half_lo<NTH>(E.buf[1]), half_hi<NTH>(E.buf[1]), c1, dc.ZERO, dc.E3.d0, dc.E3.d1, &dc);
   dadd<NTH>(dview<NTH>(E.buf[0], 1), dview<NTH>(E.buf[1], 1), dc.N);
-  int sw = 1;
-  int cur = dpow_fixed<NTH, W>(E, 0, 1, e, nl, nwin, &sw);
+}
+// Exit: the number in (buf[cur], orientation sw) times (1, 0), then the plain integer d0 + n*d1 -> out_row (4*NTH quads).
+template <int NTH>
+PAI_DEV void digit_leave_store(const DPowEnv<NTH>& E, int cur, int sw, uint32_t* out_row, bool store) {
+  const DigitEnv& dc = *E.dc;
   int oth = cur ^ 1;
   DNum x = dview<NTH>(E.buf[cur], sw);
   dmul<NTH>(half_lo<NTH>(E.buf[oth]), half_hi<NTH>(E.buf[oth]), x.d0, x.d1, dc.ONE, dc.ZERO, &dc);
   digits_to_plain<NTH>(E.buf[cur], dview<NTH>(E.buf[oth], 1), dc.N);
   if (store) store_row(out_row, E.buf[cur], 4 * NTH);
+}
+
+// c^k mod n^2 with per-element exponents in digit form (EncryptedNumber._raw_mul, phe/paillier.py:749-751).
+//   base row: plain ciphertext, 2*NTH tiles = c_0 + c_1*R;  e: exponent limbs of this element; nwin uniform.
+template <int NTH, int W>
+PAI_DEV void prog_powmod_digit(DPowEnv<NTH>& E, const uint32_t* base_row, const uint32_t* e, int nl, int nwin,
+                               uint32_t* out_row, bool store) {
+  digit_enter<NTH>(E, base_row);
+  int sw = 1;
+  int cur = dpow_fixed<NTH, W>(E, 0, 1, e, nl, nwin, &sw);
+  digit_leave_store<NTH>(E, cur, sw, out_row, store);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Plaintext matrix (CSR) times ciphertext vector (pai_raw_matvec): out[j] = prod_t T[col_t, sign_t] ^ mag_t mod n^2.
+// Window tables are built once per base and shared by every row.  Slot s < ncols holds the powers of c[s], slot
+// ncols + i those of c[i]^-1 (built only for columns used with a negative scalar).  Entry k = 1 .. 2^w - 1 of a slot is
+// base^k * R in digit form, [d0 | d1] with stride 1, at quad (s * (2^w - 1) + k - 1) * 4*NTH of the table.
+template <int NTH>
+PAI_DEV DNum mv_entry(const u4* tbl, long slot, int w, uint32_t k) {
+  Opnd o;
+  o.p = (u4*)tbl + ((size_t)slot * ((1u << w) - 1u) + (k - 1u)) * 4 * NTH;
+  o.s = 1;
+  return dview<NTH>(o, 0);
+}
+template <int NTH>
+PAI_DEV void dnum_copy(const DNum& dst, const DNum& src) {
+  big_copy<NTH>(dst.d0, src.d0);
+  big_copy<NTH>(dst.d1, src.d1);
+}
+
+// the 2^w - 1 entries of one slot: T[1] = base * R, T[k] = T[k-1] * T[1]  (2^w - 2 products, serial)
+template <int NTH>
+PAI_DEV void prog_matvec_table(const DPowEnv<NTH>& E, const uint32_t* base_row, u4* tbl, long slot, int w) {
+  digit_enter<NTH>(E, base_row);
+  const DNum t1 = mv_entry<NTH>(tbl, slot, w, 1);
+  dnum_copy<NTH>(t1, dview<NTH>(E.buf[0], 1));
+  int cur = 0;
+  for (uint32_t k = 2; k < (1u << w); k++) {
+    DNum x = dview<NTH>(E.buf[cur], 1);
+    dmul<NTH>(half_lo<NTH>(E.buf[cur ^ 1]), half_hi<NTH>(E.buf[cur ^ 1]), x.d0, x.d1, t1.d0, t1.d1, E.dc);
+    cur ^= 1;
+    dnum_copy<NTH>(mv_entry<NTH>(tbl, slot, w, k), dview<NTH>(E.buf[cur], 1));
+  }
+}
+
+// One output row by Straus' method over the row's entries [lo, hi): the accumulator starts at one (R in digit form);
+// window wi (top down) costs w squarings (none for the top window) and one product per entry whose digit is non-zero.
+template <int NTH>
+PAI_DEV void prog_matvec_row(const DPowEnv<NTH>& E, const u4* tbl, long ncols, int w, int nwin, const int32_t* indices,
+                             const uint32_t* mag, int ml, const uint8_t* neg, long lo, long hi, uint32_t* out_row, bool store) {
+  const DigitEnv& dc = *E.dc;
+  int cur = 0, sw = 0;
+  dnum_copy<NTH>(dview<NTH>(E.buf[0], 0), dc.ONEM);
+  for (int wi = nwin - 1; wi >= 0; wi--) {
+    if (wi != nwin - 1) {
+      for (int s = 0; s < w; s++) {
+        DNum x = dview<NTH>(E.buf[cur], sw);
+        dsqr<NTH>(half_lo<NTH>(E.buf[cur ^ 1]), half_hi<NTH>(E.buf[cur ^ 1]), x.d0, x.d1, &dc);
+        cur ^= 1;
+        sw = 1;
+      }
+    }
+    for (long t = lo; t < hi; t++) {
+      const uint32_t dg = exp_digit(mag + t * ml, ml, wi * w, w);
+      if (!dg) continue;
+      const long slot = (neg && neg[t]) ? ncols + indices[t] : (long)indices[t];
+      const DNum te = mv_entry<NTH>(tbl, slot, w, dg);
+      DNum x = dview<NTH>(E.buf[cur], sw);
+      dmul<NTH>(half_lo<NTH>(E.buf[cur ^ 1]), half_hi<NTH>(E.buf[cur ^ 1]), x.d0, x.d1, te.d0, te.d1, &dc);
+      cur ^= 1;
+      sw = 1;
+    }
+  }
+  digit_leave_store<NTH>(E, cur, sw, out_row, store);
 }
 
 }  // namespace pai

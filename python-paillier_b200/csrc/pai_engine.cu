@@ -94,6 +94,30 @@ struct PowDigitBody {
   const uint32_t* gzero;
   PAI_MEM void run(u4* smem, const CtaId& id) const { cta_powmod_digit<NTH, W>(smem, id, base, exp, exp_limbs, out, batch, tbl, counter, gzero); }
 };
+// matrix-vector product (pai_raw_matvec): column flags, shared window tables, rows
+struct MatFlagBody {
+  const uint32_t* consts; int const_quads;
+  const int32_t* indices; const uint8_t* neg; long nnz; int32_t* flag;
+  PAI_MEM void run(u4*, const CtaId& id) const {
+    for (long t = (long)id.cta * id.nthr + id.tid; t < nnz; t += (long)id.ncta * id.nthr)
+      if (neg[t]) flag[indices[t]] = 1;
+  }
+};
+template <int NTH>
+struct MatTblBody {
+  const uint32_t* consts; int const_quads;
+  const uint32_t* c; const uint32_t* cinv; const int32_t* flag; long ncols, nslots; int w; u4* tbl; const uint32_t* gzero;
+  PAI_MEM void run(u4* smem, const CtaId& id) const { cta_matvec_table<NTH>(smem, id, c, cinv, flag, ncols, nslots, w, tbl, gzero); }
+};
+template <int NTH>
+struct MatRowBody {
+  const uint32_t* consts; int const_quads;
+  const u4* tbl; long ncols; int w; const int64_t* indptr; const int32_t* indices; const uint32_t* mag; int ml;
+  const uint8_t* neg; uint32_t* out; long nrows; unsigned long long* counter; const uint32_t* gzero;
+  PAI_MEM void run(u4* smem, const CtaId& id) const {
+    cta_matvec_digit<NTH>(smem, id, tbl, ncols, w, indptr, indices, mag, ml, neg, out, nrows, counter, gzero);
+  }
+};
 template <int NT>
 struct MulBody {
   const uint32_t* consts; int const_quads;
@@ -397,9 +421,12 @@ struct Counters {
 // different streams never share scratch memory (launches on ONE stream are ordered and may).  Looked up under the
 // context's mutex; lives until the context is destroyed.
 struct StreamWs {
-  DevBuf tbl, w_base, w_exp, w_flag, coop_u, red_a, red_b;
+  DevBuf tbl, w_base, w_exp, w_flag, coop_u, red_a, red_b, mv_tbl;
   Counters ctr;
-  void release() { tbl.release(); w_base.release(); w_exp.release(); w_flag.release(); coop_u.release(); red_a.release(); red_b.release(); ctr.buf.release(); }
+  void release() {
+    tbl.release(); w_base.release(); w_exp.release(); w_flag.release(); coop_u.release(); red_a.release(); red_b.release();
+    mv_tbl.release(); ctr.buf.release();
+  }
 };
 struct WsMap {
   std::map<rt_stream, StreamWs> m;
@@ -894,6 +921,56 @@ int do_powmod_digit(pai_pub* k, const uint32_t* base, const uint32_t* d_exp, int
   if (rc) return rc;
   B body{k->d_enc_consts, cq, base, d_exp, exp_limbs, out, batch, (u4*)m->ws.get(s).tbl.p, ctr, m->d_blob + dc_zero_offset(NTH)};
   return rt_launch(body, g.grid, g.nthr, g.smem, s);
+}
+
+// Window width of the matrix-vector product: the w in 1..8 with the fewest modular multiplications,
+//   tabled * (2^w - 2)  +  nrows * bits  +  nnz * ceil(bits / w)       (tables, squarings, products)
+// among the widths whose tables fit MATVEC_TABLE_BUDGET.  w = 1 needs no table products (a table entry is the base
+// itself, the size of the vector), so it is taken when nothing wider fits: the columns are never split into blocks.
+#if defined(PAI_HOSTSIM)
+const size_t MATVEC_TABLE_BUDGET = (size_t)64 << 10;       // the CPU simulation reaches w = 1 at small shapes
+#else
+const size_t MATVEC_TABLE_BUDGET = (size_t)2 << 30;
+#endif
+int matvec_window(long tabled, long nrows, long nnz, int bits, size_t entry_bytes) {
+  int best = 1;
+  double best_cost = 0;
+  for (int w = 1; w <= 8; w++) {
+    if (w > 1 && (double)tabled * ((1 << w) - 1) * (double)entry_bytes > (double)MATVEC_TABLE_BUDGET) break;
+    const double cost = (double)tabled * ((1 << w) - 2) + (double)nrows * bits + (double)nnz * ((bits + w - 1) / w);
+    if (w == 1 || cost < best_cost) { best = w; best_cost = cost; }
+  }
+  return best;
+}
+size_t matvec_entry_bytes(int NTH) { return (size_t)4 * NTH * 16; }
+
+template <int NTH>
+int do_matvec_digit(pai_pub* k, StreamWs& w, const uint32_t* c, const uint32_t* cinv, const int32_t* flag, long ncols,
+                    long nslots, int win, const int64_t* indptr, const int32_t* indices, const uint32_t* mag, int ml,
+                    const uint8_t* neg, long nnz, long nrows, uint32_t* out, rt_stream s) {
+  pai_mod* m = k->nmod;
+  const int cq = dc_pow_limbs(NTH) / 4;
+  const uint32_t* gzero = m->d_blob + dc_zero_offset(NTH);
+  int rc = 0;
+  if (nnz > 0) {
+    typedef MatTblBody<NTH> TB;
+    Geom g;
+    rc = geometry<TB>(m->device, 2 * NTH, cq, 2, nslots, g);
+    if (!rc) rc = w.mv_tbl.ensure((size_t)nslots * ((1u << win) - 1u) * matvec_entry_bytes(NTH));
+    if (rc) return rc;
+    TB tb{k->d_enc_consts, cq, c, cinv, flag, ncols, nslots, win, (u4*)w.mv_tbl.p, gzero};
+    rc = rt_launch(tb, g.grid, g.nthr, g.smem, s);
+    if (rc) return rc;
+  }
+  typedef MatRowBody<NTH> RB;
+  Geom g;
+  rc = geometry<RB>(m->device, 2 * NTH, cq, 2, nrows, g);
+  if (rc) return rc;
+  unsigned long long* ctr = nullptr;
+  rc = w.ctr.take(s, &ctr);
+  if (rc) return rc;
+  RB rb{k->d_enc_consts, cq, (const u4*)w.mv_tbl.p, ncols, win, indptr, indices, mag, ml, neg, out, nrows, ctr, gzero};
+  return rt_launch(rb, g.grid, g.nthr, g.smem, s);
 }
 
 template <int NTP>
@@ -1598,6 +1675,56 @@ int pai_raw_dot(pai_pub* k, const uint32_t* d_a, const uint32_t* d_s, uint32_t* 
   }
   CtxLock lock2_(m->mu);
   DISPATCH_NT(m->NT, rc = do_reduce_mul<NT>(m, (const uint32_t*)w.red_b.p, nrows, d_out, s));
+  return rc;
+}
+
+int pai_raw_matvec_window(pai_pub* k, long ncols, long nrows, long nnz, int mag_bits, int with_neg) {
+  if (!k || ncols < 0 || nrows < 0 || nnz < 0 || mag_bits < 0) { g_err = "bad argument"; return PAI_E_ARG; }
+  const long tabled = with_neg ? 2 * ncols : ncols;
+  return matvec_window(tabled, nrows, nnz, mag_bits, matvec_entry_bytes(k->nmod->NT));
+}
+
+int pai_raw_matvec(pai_pub* k, const uint32_t* d_c, long ncols, const int64_t* d_indptr, const int32_t* d_indices,
+                   const uint32_t* d_mag, int mag_limbs, int mag_bits, const uint8_t* d_neg, long nnz, long nrows,
+                   uint32_t* d_out, int32_t* d_status, void* stream) {
+  DeviceGuard device_guard_; (void)device_guard_;
+  if (!k || ncols < 0 || nrows < 0 || nnz < 0 || mag_limbs < 1 || mag_bits < 0 || mag_bits > 32 * mag_limbs ||
+      (nrows > 0 && (!d_indptr || !d_out)) || (nnz > 0 && (!d_c || !d_indices || !d_mag || ncols < 1))) {
+    g_err = "bad argument";
+    return PAI_E_ARG;
+  }
+  CtxLock lock_(k->mu);
+  rt_stream s = (rt_stream)stream;
+  int rc = rt_set_device(k->nsq->device);
+  if (rc) return rc;
+  StreamWs& w = k->ws.get(s);
+  const bool inverses = d_neg && nnz > 0;
+  if (d_status && ncols > 0 && !inverses) rc = rt_memset(d_status, 0, (size_t)ncols * 4, s);
+  if (rc || nrows == 0) return rc;
+  const int lc = 2 * k->ln;
+  const int bits = mag_bits ? mag_bits : 32 * mag_limbs;
+  const long nslots = inverses ? 2 * ncols : ncols;
+  const int win = matvec_window(nslots, nrows, nnz, bits, matvec_entry_bytes(k->nmod->NT));
+  int32_t* flag = nullptr;
+  const uint32_t* cinv = nullptr;
+  if (inverses) {   // 1. columns used with a negative scalar, 2. their inverses (the others are copied)
+    rc = w.w_flag.ensure((size_t)ncols * 4 * 2);
+    if (!rc) rc = w.w_base.ensure((size_t)ncols * lc * 4);
+    if (!rc) rc = rt_memset(w.w_flag.p, 0, (size_t)ncols * 4, s);
+    if (rc) return rc;
+    flag = (int32_t*)w.w_flag.p;
+    int32_t* status = d_status ? d_status : flag + ncols;
+    MatFlagBody fb{nullptr, 0, d_indices, d_neg, nnz, flag};
+    rc = rt_launch(fb, (int)std::min((nnz + 127) / 128, 65535L), 128, 0, s);
+    if (rc) return rc;
+    pai_mod* m = k->nsq;
+    DISPATCH_NT(m->NT, rc = do_invert_flagged<NT>(m, d_c, flag, (uint32_t*)w.w_base.p, status, ncols, s));
+    if (rc) return rc;
+    cinv = (const uint32_t*)w.w_base.p;
+  }
+  // 3. shared window tables, 4. one thread per row
+  DISPATCH_NTH(k->nmod->NT, rc = do_matvec_digit<NTH>(k, w, d_c, cinv, flag, ncols, nslots, win, d_indptr, d_indices, d_mag,
+                                                      mag_limbs, inverses ? d_neg : nullptr, nnz, nrows, d_out, s));
   return rc;
 }
 

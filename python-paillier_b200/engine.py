@@ -65,6 +65,9 @@ SYMBOLS = {
     "pai_miller_rabin": (ctypes.c_int, [_vp, ctypes.c_int, _vp, ctypes.c_int, _vp, ctypes.c_long, ctypes.c_int, _vp]),
     "pai_raw_sum": (ctypes.c_int, [_vp, _vp, ctypes.c_long, _vp, _vp]),
     "pai_raw_dot": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, ctypes.c_long, _vp]),
+    "pai_raw_matvec": (ctypes.c_int, [_vp, _vp, ctypes.c_long, _vp, _vp, _vp, ctypes.c_int, ctypes.c_int, _vp, ctypes.c_long,
+                                      ctypes.c_long, _vp, _vp, _vp]),
+    "pai_raw_matvec_window": (ctypes.c_int, [_vp, ctypes.c_long, ctypes.c_long, ctypes.c_long, ctypes.c_int, ctypes.c_int]),
     "pai_priv_create": (ctypes.c_int, [_vp, _vp, ctypes.c_int, ctypes.c_int, ctypes.POINTER(_vp)]),
     "pai_priv_destroy": (ctypes.c_int, [_vp]),
     "pai_priv_n_limbs": (ctypes.c_int, [_vp]),
@@ -391,6 +394,20 @@ class PublicContext:
     def raw_dot_dev(self, d_a, d_s, d_out, d_status, batch, stream=None):
         """d_out[0] = prod_i d_a[i]^d_s[i] mod n^2 (encrypted dot product with plaintext scalars)."""
         self.eng.check(self.eng.lib.pai_raw_dot(self.h, _ptr(d_a), _ptr(d_s), _ptr(d_out), _ptr(d_status), batch, _ptr(stream)))
+
+    def raw_matvec_dev(self, d_c, ncols, d_indptr, d_indices, d_mag, mag_limbs, mag_bits, d_neg, nnz, nrows, d_out,
+                       d_status, stream=None):
+        """d_out[j] = prod over the CSR entries t of row j of (d_neg[t] ? d_c[col]^-1 : d_c[col]) ^ d_mag[t] mod n^2
+        (plaintext matrix times ciphertext vector, include/paillier_b200.h pai_raw_matvec).  d_neg may be None."""
+        self.eng.check(self.eng.lib.pai_raw_matvec(self.h, _ptr(d_c), ncols, _ptr(d_indptr), _ptr(d_indices), _ptr(d_mag),
+                                                   mag_limbs, mag_bits, _ptr(d_neg), nnz, nrows, _ptr(d_out),
+                                                   _ptr(d_status), _ptr(stream)))
+
+    def matvec_window(self, ncols, nrows, nnz, bits, with_neg):
+        """The window width raw_matvec_dev picks for these shapes."""
+        w = int(self.eng.lib.pai_raw_matvec_window(self.h, ncols, nrows, nnz, bits, 1 if with_neg else 0))
+        self.eng.check(min(w, 0))
+        return w
 
     # ---- host-array API (numpy uint32 limb matrices), synchronous
     def encrypt_host(self, m, r):

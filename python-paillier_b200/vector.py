@@ -127,13 +127,11 @@ def _limbs_from_signed(int_rep, n, ln):
     return out
 
 
-def encode_batch(public_key, values, precision=None, max_exponent=None):
-    """Encode a sequence like EncodedNumber.encode does element by element.
-    Returns (limbs [B, n_limbs] uint32 of the encodings, exponents [B] int64)."""
-    ctx = public_key.engine_context()
-    ln = ctx.n_limbs
+def _encode_fast(public_key, values, max_exponent=None):
+    """The numpy fast path of encode_batch: (signed integer representations [B] int64, exponents [B] int64), or None
+    when the values need the per-element path."""
     arr = None
-    if precision is None and public_key.n.bit_length() > 80:
+    if public_key.n.bit_length() > 80:
         if isinstance(values, np.ndarray) and values.dtype in (np.float64, np.int64, np.int32):
             arr = values
         elif len(values) and all(type(v) is float for v in values):
@@ -149,12 +147,23 @@ def encode_batch(public_key, values, precision=None, max_exponent=None):
             exps = np.minimum(exps, np.asarray(max_exponent, dtype=np.int64))
         shift = lsb - 4 * exps
         if (shift <= 9).all():                                        # |int_rep| < 2^62
-            int_rep = np.left_shift(mant, shift)
-            return _limbs_from_signed(int_rep, public_key.n, ln), exps
+            return np.left_shift(mant, shift), exps
     elif arr is not None and arr.dtype != np.float64:
         exps = np.zeros(arr.shape[0], dtype=np.int64)
         if max_exponent is None or (np.asarray(max_exponent) >= 0).all():
-            return _limbs_from_signed(arr.astype(np.int64), public_key.n, ln), exps
+            return arr.astype(np.int64), exps
+    return None
+
+
+def encode_batch(public_key, values, precision=None, max_exponent=None):
+    """Encode a sequence like EncodedNumber.encode does element by element.
+    Returns (limbs [B, n_limbs] uint32 of the encodings, exponents [B] int64)."""
+    ctx = public_key.engine_context()
+    ln = ctx.n_limbs
+    if precision is None:
+        fast = _encode_fast(public_key, values, max_exponent)
+        if fast is not None:
+            return _limbs_from_signed(fast[0], public_key.n, ln), fast[1]
     if isinstance(max_exponent, (list, tuple, np.ndarray)):
         mex = [int(x) for x in max_exponent]
     else:
@@ -208,6 +217,92 @@ def decode_batch(public_key, limbs, exponents):
         for i, enc in zip(slow, encs):
             out[i] = EncodedNumber(public_key, enc, int(exps[i])).decode()
     return out
+
+
+# ------------------------------------------------------------------------------------------------------
+# Host preparation of EncryptedVector.rmatmul: sign-and-magnitude scalars with the exponent alignment folded in.
+def _is_sparse(X):
+    try:
+        import scipy.sparse as sp
+    except ImportError:
+        return False
+    return sp.issparse(X)
+
+
+def _plain_values(a):
+    """Matrix entries as encode_batch takes them: float64 for every float dtype and int64 for integer and bool dtypes that
+    fit it (both give the encodings EncodedNumber.encode gives their Python values), Python objects otherwise."""
+    k = a.dtype.kind
+    if k == "f":
+        return a.astype(np.float64)
+    if k in "bi" or (k == "u" and (a.size == 0 or int(a.max()) < 2 ** 63)):
+        return a.astype(np.int64)
+    return a.astype(object)
+
+
+def _signed_encodings(public_key, values):
+    """encode_batch of `values` as sign and magnitude: (neg [B] bool, mag, exponents [B] int64).  mag is a uint64 array on
+    encode_batch's fast path (|int_rep| < 2^62), else a list of Python ints from the per-element path; an encoding s
+    is negative where s >= n - max_int, with magnitude n - s (phe/paillier.py:742-749)."""
+    fast = _encode_fast(public_key, values)
+    if fast is not None:
+        int_rep, exps = fast
+        return int_rep < 0, np.abs(int_rep).astype(np.uint64), exps
+    limbs, exps = encode_batch(public_key, values)
+    n, thr = public_key.n, public_key.n - public_key.max_int
+    encs = limbs_to_ints(limbs)
+    return np.array([e >= thr for e in encs], dtype=bool), [n - e if e >= thr else e for e in encs], exps
+
+
+def _bitlen64(x):
+    """bit lengths of a uint64 array (exact: each 32-bit half converts to float64 without rounding)"""
+    def bl32(v):
+        return np.frexp(v.astype(np.float64))[1].astype(np.int64)
+    hi = x >> np.uint64(32)
+    return np.where(hi > 0, 32 + bl32(hi), bl32(x & np.uint64(0xffffffff)))
+
+
+def _aligned_magnitudes(public_key, mag, delta):
+    """|k| * BASE^delta of every entry as a limb matrix: (limbs per row L, bit bound, uint32 [B, L]).  On the fast path
+    the shift by 4*delta bits is done on numpy words; a product above max_int raises dot()'s ValueError."""
+    max_int = public_key.max_int
+    shift = delta.astype(np.int64) * int(EncodedNumber.LOG2_BASE)
+
+    def too_big(m, s):
+        raise ValueError('Integer needs to be within +/- %d but got %d' % (max_int, m << s))
+    if isinstance(mag, np.ndarray):
+        tb = _bitlen64(mag) + shift
+        for i in np.nonzero(tb >= max_int.bit_length())[0].tolist():       # at or above the bound: exact check
+            if int(mag[i]) << int(shift[i]) > max_int:
+                too_big(int(mag[i]), int(shift[i]))
+        bits = int(tb.max()) if len(tb) else 1
+        L = max(1, (bits + 31) // 32)
+        q, r = shift // 32, (shift % 32).astype(np.uint64)
+        m32 = np.uint64(0xffffffff)
+        a, b = (mag & m32) << r, (mag >> np.uint64(32)) << r                 # each below 2^63
+        # words q, q+1, q+2 of every row through a flat index (two spare columns: words above the bound are zero)
+        out = np.zeros((len(mag), L + 2), dtype=np.uint32)
+        flat = out.reshape(-1)
+        at = np.arange(len(mag), dtype=np.int64) * (L + 2) + q
+        flat[at] = (a & m32).astype(np.uint32)
+        flat[at + 1] = ((a >> np.uint64(32)) | (b & m32)).astype(np.uint32)
+        flat[at + 2] = (b >> np.uint64(32)).astype(np.uint32)
+        out = np.ascontiguousarray(out[:, :L])
+        return L, max(bits, 1), out
+    vals = []
+    for m, s in zip(mag, shift.tolist()):
+        if m << s > max_int:
+            too_big(m, s)
+        vals.append(m << s)
+    bits = max([v.bit_length() for v in vals] + [1])
+    L = (bits + 31) // 32
+    return L, bits, ints_to_limbs(vals, L)
+
+
+def _arr_to_dev(arr, ctx):
+    """numpy array (any dtype) -> torch tensor on the context's GPU (host tensor for the simulation build)"""
+    t = _torch().from_numpy(np.ascontiguousarray(arr))
+    return t if ctx.eng.simulated else t.to("cuda:%d" % ctx.device)
 
 
 class EncryptedVector(object):
@@ -363,8 +458,16 @@ class EncryptedVector(object):
         return EncryptedVector(self.public_key, limbs, new_exps.copy(), obfuscated=self._obfuscated and not len(idx))
 
     def __add__(self, other):
+        from .paillier import EncryptedNumber
         ctx = self.public_key.engine_context()
         torch = _torch()
+        if isinstance(other, EncryptedNumber):
+            # broadcast: one row uploaded and expanded on the device, then the vector + vector path (exponent alignment)
+            if self.public_key != other.public_key:
+                raise ValueError("Attempted to add numbers encrypted against different public keys!")
+            row = _to_dev(ints_to_limbs([other.ciphertext(be_secure=False) % self.public_key.nsquare], ctx.c_limbs), ctx)
+            other = EncryptedVector(self.public_key, row.expand(len(self), -1).contiguous(),
+                                    np.full(len(self), other.exponent, dtype=np.int64))
         if isinstance(other, EncryptedVector):
             if self.public_key != other.public_key:
                 raise ValueError("Attempted to add numbers encrypted against different public keys!")
@@ -510,6 +613,91 @@ class EncryptedVector(object):
     def dot_chain(self, scalars):
         """The round-1 form of dot(): one raw_mul launch, then sum_chain()."""
         return (self * scalars).sum_chain()
+
+    def rmatmul(self, X):
+        """X @ self for a plaintext matrix X of shape [N, len(self)] -> EncryptedVector of length N, in one fused product
+        on the device (pai_raw_matvec): window tables of every ciphertext are built once and shared by all rows, and
+        each row runs one squaring chain for all its entries.  This is the encrypted scoring of
+        examples/logistic_regression_encrypted_model.py:170-180 for a whole matrix; ``v.rmatmul(X) + enc_b`` adds the
+        intercept.
+
+        X is a 2-D numpy array (float or int) or any scipy.sparse matrix or array.
+          - dense X: row j equals ``self.dot(X[j])``, the same ciphertext with the same exponent (the lowest exponent
+            over ALL entries of the row, zeros included; zero scalars contribute nothing).
+          - sparse X: row j equals the reference's loop ``score += x[0, i] * w[i]`` over ``x.nonzero()`` without an
+            intercept (explicitly stored zeros are ignored); an empty row is the ciphertext 1 with exponent 0.
+        Exponents are aligned inside the scalars as in dot(), with the same ValueError when |k| * BASE^delta exceeds
+        max_int; a ciphertext used with a negative scalar that has no inverse mod n^2 raises ZeroDivisionError.  The
+        result is not obfuscated.
+
+        ``X @ v`` reaches this method for numpy X.  ``scipy_matrix @ v`` does NOT: scipy converts v with
+        np.asanyarray first, so scipy users call ``v.rmatmul(X)``.  A single row is latency bound here (one thread
+        per row): use dot() for a 1 x d product."""
+        pk = self.public_key
+        ctx = pk.engine_context()
+        torch = _torch()
+        sparse = _is_sparse(X)
+        if not sparse:
+            X = np.asarray(X)
+            if X.ndim == 1:
+                raise ValueError("rmatmul needs a 2-D matrix; use dot() for a 1-D vector of scalars")
+        if X.ndim != 2:
+            raise ValueError("rmatmul needs a 2-D matrix")
+        nrows, ncols = (int(x) for x in X.shape)
+        if ncols != len(self):
+            raise ValueError("matrix has %d columns, the vector %d elements" % (ncols, len(self)))
+        if sparse:
+            X = X.tocsr(copy=True)
+            X.sum_duplicates()
+            X.eliminate_zeros()                           # x.nonzero() skips explicitly stored zeros
+            indptr = X.indptr.astype(np.int64)
+            cols = X.indices.astype(np.int64)
+            vals = _plain_values(X.data)
+        else:
+            indptr = np.arange(nrows + 1, dtype=np.int64) * ncols
+            cols = np.tile(np.arange(ncols, dtype=np.int64), nrows)
+            vals = _plain_values(X.reshape(-1))
+        rows = np.repeat(np.arange(nrows, dtype=np.int64), np.diff(indptr))
+        neg, mag, exps = _signed_encodings(pk, vals)
+        # row exponent: the lowest exponent among the row's entries (dense: zeros included); empty rows: 0
+        texp = self.exponents[cols] + exps
+        row_exp = np.zeros(nrows, dtype=np.int64)
+        filled = np.diff(indptr) > 0
+        if filled.any():
+            row_exp[filled] = np.minimum.reduceat(texp, indptr[:-1][filled])
+        delta = texp - row_exp[rows]
+        keep = np.nonzero(mag != 0 if isinstance(mag, np.ndarray) else np.array([m != 0 for m in mag], dtype=bool))[0]
+        rows, cols, neg, delta = rows[keep], cols[keep], neg[keep], delta[keep]
+        mag = mag[keep] if isinstance(mag, np.ndarray) else [mag[i] for i in keep.tolist()]
+        mag_limbs, mag_bits, m_limbs = _aligned_magnitudes(pk, mag, delta)
+        # rows by decreasing length, so that the rows of a warp are about equally long
+        counts = np.bincount(rows, minlength=nrows)
+        order = np.argsort(-counts, kind="stable")
+        s_indptr = np.zeros(nrows + 1, dtype=np.int64)
+        np.cumsum(counts[order], out=s_indptr[1:])
+        starts = np.zeros(nrows, dtype=np.int64)
+        np.cumsum(counts[:-1], out=starts[1:])
+        shift = np.repeat(starts[order] - s_indptr[:-1], counts[order])
+        perm = slice(None) if not shift.any() else np.arange(len(keep), dtype=np.int64) + shift
+        nnz = len(keep)
+        dev = self.limbs.device
+        d_indptr = _arr_to_dev(s_indptr, ctx)
+        d_indices = _arr_to_dev(cols[perm].astype(np.int32), ctx)
+        d_mag = _to_dev(m_limbs[perm], ctx)
+        any_neg = bool(neg.any())
+        d_neg = _arr_to_dev(neg[perm].astype(np.uint8), ctx) if any_neg else None
+        out = torch.empty((nrows, ctx.c_limbs), dtype=torch.int32, device=dev)
+        status = torch.zeros((max(ncols, 1),), dtype=torch.int32, device=dev)
+        if nrows:
+            ctx.raw_matvec_dev(self.limbs, ncols, d_indptr, d_indices, d_mag, mag_limbs, mag_bits, d_neg, nnz, nrows, out,
+                               status, stream=_stream(ctx))
+            if any_neg and bool(status.any().item()):
+                raise ZeroDivisionError('invert() no inverse exists')
+        res = torch.empty_like(out)
+        res.index_copy_(0, _arr_to_dev(order, ctx), out)
+        return EncryptedVector(pk, res, row_exp)
+
+    __rmatmul__ = rmatmul
 
     # ------------------------------------------------------------------ wire format
     def to_json(self, be_secure=True):
