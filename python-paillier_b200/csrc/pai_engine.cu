@@ -387,24 +387,40 @@ std::vector<uint32_t> sliding_program(const limbs_t& e, int w) {
   return prog;
 }
 
+// Device memory a context owns.  It knows its size, so a context holding key material can zero it before the free
+// (`release(true)`: a memset and a sync on the current device, which the destroy functions set first).
+template <class T = void>
 struct DevBuf {
-  void* p = nullptr; size_t bytes = 0;
+  T* p = nullptr; size_t bytes = 0;
   int ensure(size_t need) {
     if (need <= bytes) return 0;
-    rt_free(p); p = nullptr; bytes = 0;
-    int rc = rt_malloc(&p, need);
+    release();
+    int rc = rt_malloc((void**)&p, need);
     if (rc) return rc;
     bytes = need;
     return 0;
   }
-  void release() { rt_free(p); p = nullptr; bytes = 0; }
+  void release(bool wipe = false) {
+    if (wipe && p) { rt_memset(p, 0, bytes, 0); rt_sync(0); }
+    rt_free(p); p = nullptr; bytes = 0;
+  }
+};
+// a temporary device buffer, freed on every return path
+struct TmpBuf {
+  void* p = nullptr;
+  TmpBuf() = default;
+  TmpBuf(const TmpBuf&) = delete;
+  TmpBuf& operator=(const TmpBuf&) = delete;
+  ~TmpBuf() { rt_free(p); }
+  int alloc(size_t bytes) { return rt_malloc(&p, bytes); }
+  uint32_t* u32() const { return (uint32_t*)p; }
 };
 
 // work counters of the persistent kernels: a ring of zero-initialised 64-bit counters per (context, stream);
 // each launch takes the next one and re-zeroes it on the launch stream first (launches on one stream are
 // ordered, so a counter is never re-armed while a previous kernel on that stream still uses it).
 struct Counters {
-  DevBuf buf; int next = 0;
+  DevBuf<> buf; int next = 0;
   int take(rt_stream s, unsigned long long** out) {
     int rc = buf.ensure(64 * 8);
     if (rc) return rc;
@@ -421,17 +437,16 @@ struct Counters {
 // different streams never share scratch memory (launches on ONE stream are ordered and may).  Looked up under the
 // context's mutex; lives until the context is destroyed.
 struct StreamWs {
-  DevBuf tbl, w_base, w_exp, w_flag, coop_u, red_a, red_b, mv_tbl;
+  DevBuf<> tbl, w_base, w_exp, w_flag, coop_u, red_a, red_b, mv_tbl;
   Counters ctr;
-  void release() {
-    tbl.release(); w_base.release(); w_exp.release(); w_flag.release(); coop_u.release(); red_a.release(); red_b.release();
-    mv_tbl.release(); ctr.buf.release();
+  void release(bool wipe) {
+    for (DevBuf<>* b : {&tbl, &w_base, &w_exp, &w_flag, &coop_u, &red_a, &red_b, &mv_tbl, &ctr.buf}) b->release(wipe);
   }
 };
 struct WsMap {
   std::map<rt_stream, StreamWs> m;
   StreamWs& get(rt_stream s) { return m[s]; }
-  void release() { for (auto& kv : m) kv.second.release(); m.clear(); }
+  void release(bool wipe = false) { for (auto& kv : m) kv.second.release(wipe); m.clear(); }
 };
 typedef std::lock_guard<std::recursive_mutex> CtxLock;
 
@@ -455,28 +470,64 @@ int geometry(int device, int NT, int const_quads, int nbuf, long batch, Geom& g)
   g.nthr = nthr; g.smem = smem; g.grid = (int)std::max(1L, std::min(chunks, maxgrid));
   return 0;
 }
-size_t table_bytes(const Geom& g, int NT, int W) { return (size_t)g.grid * ((size_t)1 << W) * 2 * NT * g.nthr * 16; }
+long wave_rows(const Geom& g) { return (long)g.grid * g.nthr; }
+
+// What a persistent kernel with a window table needs from its launcher, stated once per body: operand tiles, constant
+// quads, operand buffers and table entries per thread (2 * tiles quads each)
+struct Shape { int nt, cq, nbuf; long entries; };
+// rows one full grid of B holds (0 when B cannot be resident)
+template <class B>
+long wave_of(int device, const Shape& sh) {
+  Geom g;
+  return geometry<B>(device, sh.nt, sh.cq, sh.nbuf, 1L << 40, g) ? 0 : wave_rows(g);
+}
+// geometry, the window-table workspace, a work counter and the launch of a persistent kernel B over `batch` rows;
+// make(tbl, counter) builds the body
+template <class B, class Make>
+int launch_persistent(int device, StreamWs& w, const Shape& sh, long batch, rt_stream s, Make make) {
+  Geom g;
+  int rc = geometry<B>(device, sh.nt, sh.cq, sh.nbuf, batch, g);
+  if (!rc) rc = w.tbl.ensure((size_t)g.grid * sh.entries * 2 * sh.nt * g.nthr * 16);
+  unsigned long long* ctr = nullptr;
+  if (!rc) rc = w.ctr.take(s, &ctr);
+  if (rc) return rc;
+  return rt_launch(make((u4*)w.tbl.p, ctr), g.grid, g.nthr, g.smem, s);
+}
+// a one-thread setup kernel (per key): `scratch_bytes` of device scratch, one 32-thread CTA, waited for; make(scratch)
+// builds the body
+template <class Make>
+int run_setup(size_t scratch_bytes, rt_stream s, Make make) {
+  TmpBuf scratch;
+  int rc = scratch.alloc(scratch_bytes);
+  if (!rc) rc = rt_launch(make(scratch.u32()), 1, 32, 0, s);
+  if (!rc) rc = rt_sync(s);
+  return rc;
+}
 
 }  // namespace
+
+// kernel family of a context; the values are the codes pai_*_kernel_path returns
+enum Family { FULL = 0, DIGIT = 1, TC = 2 };
 
 // ------------------------------------------------------------------------------------------------
 struct pai_mod {
   int device = 0, NT = 0, L = 0;
-  uint32_t* d_blob = nullptr;       // mc_limbs(NT) (+ extra room requested by the owner)
+  DevBuf<uint32_t> d_blob;          // mc_limbs(NT) (+ extra room requested by the owner)
   limbs_t h_N;                      // padded modulus
-  DevBuf tmp_a, tmp_b, tmp_o, tmp_s, tmp_e;   // staging of the host-pointer entry points (used under `mu`, stream 0)
+  DevBuf<> tmp_a, tmp_b, tmp_o, tmp_s, tmp_e;   // staging of the host-pointer entry points (used under `mu`, stream 0)
   WsMap ws;                         // per-stream workspaces
   std::recursive_mutex mu;          // serialises host threads on this context (recursive: coop constants are built
                                     // through the context's own entry points)
-  // warp-per-ciphertext layout (pai_coop.cuh), built on first use: [ N | R^2 mod N | R^3 mod N ], R = 2^(32*32*coopK)
-  uint32_t* d_coop = nullptr; int coopK = 0; uint32_t coop_n0inv = 0; bool coop_building = false;
-  uint32_t* d_corr = nullptr;       // correction rows R^(2^i + 1) mod N of the product reduction (cta_reduce_mul), built on first use
+  // warp-per-ciphertext layout (pai_coop.cuh), built on first use (then coopK != 0): [ N | R^2 mod N | R^3 mod N ],
+  // R = 2^(32*32*coopK)
+  DevBuf<uint32_t> d_coop; int coopK = 0; uint32_t coop_n0inv = 0; bool coop_building = false;
+  DevBuf<uint32_t> d_corr;          // correction rows R^(2^i + 1) mod N of the product reduction (cta_reduce_mul), built on first use
 };
 struct pai_pub {
   pai_mod* nsq = nullptr;           // modulus n^2; its blob is followed by n (4*NT limbs) for encrypt
   int ln = 0;                       // limbs of n (= 4*NT)
   uint32_t* d_nth = nullptr;        // [ n | n - max_int ]  (ln limbs each) for raw_mul's branch test
-  DevBuf h_m, h_r, h_c, h_s;        // staging of the host-pointer entry points (under `mu`)
+  DevBuf<> h_m, h_r, h_c, h_s;      // staging of the host-pointer entry points (under `mu`)
   WsMap ws;                         // per-stream intermediates of raw_mul / reductions
   std::recursive_mutex mu;
   limbs_t h_n;
@@ -484,29 +535,27 @@ struct pai_pub {
   int nops = 0, nodd = 0;
   pai_mod* nmod = nullptr;          // modulus n with the digit-form constants appended (pai_digit.cuh)
   uint32_t* d_enc_consts = nullptr; // compact constant area of the encrypt kernel (dc_enc_limbs)
-  bool use_digit = true;            // PAI_ENCRYPT_PATH=full selects the full-width Montgomery path instead
-  uint8_t* d_tc = nullptr;          // tensor-core path: [ band(N') | band(n) ] (pai_tc.cuh); null when not supported
-  bool use_tc = false;              // PAI_TC=2 enables it
-  int tc_stagger = 0;               // start-up delay (cycles) of the second thread group
+  Family family = DIGIT;            // of encrypt and raw_mul (pick_family)
+  uint8_t* d_tc = nullptr;          // family TC only: [ band(N') | band(n) ] (pai_tc.cuh)
+  int tc_stagger = 0;               // family TC: start-up delay (cycles) of the second thread group
   long wave = 0;                    // ciphertexts per wave of the throughput encrypt kernel (lazily measured)
 };
 struct pai_priv {
   int device = 0, NTP = 0;
   pai_mod *p2 = nullptr, *q2 = nullptr, *p1 = nullptr, *q1 = nullptr;
-  uint32_t* d_consts = nullptr;     // [ P side | Q side | pinvqM ]  (full-width path, also used to derive hp/hq)
+  DevBuf<uint32_t> d_consts;        // [ P side | Q side | pinvqM ]  (full-width path, also used to derive hp/hq)
   pai_mod *pd = nullptr, *qd = nullptr;   // p, q with digit-form constants (pai_digit.cuh)
-  uint32_t* d_dconsts = nullptr;    // digit path: [ P: dblob(p) | hM | e ][ Q: ... ][ pinvqM ]
-  bool use_digit = true;
-  uint8_t* d_tc = nullptr;          // tensor-core path: [ band(p') | band(p) | band(q') | band(q) ]; null when not supported
-  bool use_tc = false;
+  DevBuf<uint32_t> d_dconsts;       // digit path: [ P: dblob(p) | hM | e ][ Q: ... ][ pinvqM ]
+  Family family = DIGIT;            // of decrypt (pick_family)
+  DevBuf<uint8_t> d_tc;             // family TC only: [ band(p') | band(p) | band(q') | band(q) ]
   int tc_stagger = 0;
   int nwin_p = 0, nwin_q = 0;
   limbs_t h_p, h_q, h_pinv, h_hp, h_hq;   // 16*NTP limbs each (padded)
-  DevBuf h_c, h_m;                  // staging of pai_decrypt_host (under `mu`)
+  DevBuf<> h_c, h_m;                // staging of pai_decrypt_host (under `mu`)
   WsMap ws;                         // per-stream window tables, counters, warp-path intermediates
   std::recursive_mutex mu;
   long wave = 0;                    // ciphertexts per wave of the throughput decrypt kernel (lazily measured)
-  uint32_t* d_coop_e = nullptr;     // [ p - 1 | q - 1 ] (8*NTP limbs each) for the warp-per-ciphertext path
+  DevBuf<uint32_t> d_coop_e;        // [ p - 1 | q - 1 ] (8*NTP limbs each) for the warp-per-ciphertext path
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -570,23 +619,24 @@ namespace {
 
 // tile counts the tensor-core kernels are instantiated for (DISPATCH_TC), up to `max_tiles`
 bool tc_supported(int tiles, int max_tiles) { return (tiles == 2 || tiles == 4 || tiles == 6 || tiles == 8 || tiles == 12) && tiles <= max_tiles; }
-// PAI_TC=2 selects the tensor-core kernels wherever they exist; by default the integer-pipe digit kernels run, which
-// measure faster on the H100 at every key size both families cover (DESIGN.md section 4)
-bool tc_wanted() {
-  const char* e = getenv("PAI_TC");
-  return e && std::string(e) == "2";
+// `path_var`=full (PAI_ENCRYPT_PATH / PAI_DECRYPT_PATH) selects the full-width Montgomery kernels; otherwise PAI_TC=2
+// selects the tensor-core kernels where they cover the key (`tc_ok`).  By default the integer-pipe digit kernels run,
+// which measure faster on the H100 at every key size both families cover (DESIGN.md section 4).
+Family pick_family(const char* path_var, bool tc_ok) {
+  const char* e = getenv(path_var);
+  if (e && std::string(e) == "full") return FULL;
+  const char* tc = getenv("PAI_TC");
+  return tc_ok && tc && std::string(tc) == "2" ? TC : DIGIT;
+}
+// start-up delay (cycles) of the second thread group of the tensor-core kernels
+int tc_stagger_cycles() {
+  const char* st = getenv("PAI_TC_STAGGER");
+  return st && *st ? atoi(st) : 40000;
 }
 
 template <int NT>
 int do_setup(pai_mod* m, rt_stream s) {
-  void* scratch = nullptr;
-  int rc = rt_malloc(&scratch, (size_t)3 * 8 * NT * 4);
-  if (rc) return rc;
-  SetupBody<NT> b{nullptr, 0, m->d_blob, (uint32_t*)scratch};
-  rc = rt_launch(b, 1, 32, 0, s);
-  if (!rc) rc = rt_sync(s);
-  rt_free(scratch);
-  return rc;
+  return run_setup((size_t)3 * 8 * NT * 4, s, [&](uint32_t* scratch) { return SetupBody<NT>{nullptr, 0, m->d_blob.p, scratch}; });
 }
 
 // create a modulus context; extra_limbs of device room are left after the blob
@@ -604,21 +654,25 @@ int mod_create_impl(const uint32_t* modulus, int limbs, int device, int force_nt
   if (!m) return PAI_E_ARG;
   m->device = device; m->NT = NT; m->L = 8 * NT;
   m->h_N = padded(modulus, eff, m->L);
-  rc = rt_malloc((void**)&m->d_blob, ((size_t)mc_limbs(NT) + extra_limbs) * 4);
-  if (!rc) rc = rt_memset(m->d_blob, 0, ((size_t)mc_limbs(NT) + extra_limbs) * 4, 0);
-  if (!rc) rc = rt_h2d(m->d_blob, m->h_N.data(), (size_t)m->L * 4, 0);
+  rc = m->d_blob.ensure(((size_t)mc_limbs(NT) + extra_limbs) * 4);
+  if (!rc) rc = rt_memset(m->d_blob.p, 0, m->d_blob.bytes, 0);
+  if (!rc) rc = rt_h2d(m->d_blob.p, m->h_N.data(), (size_t)m->L * 4, 0);
   if (!rc) { DISPATCH_NT(NT, rc = do_setup<NT>(m, 0)); }
-  if (rc) { rt_free(m->d_blob); delete m; return rc; }
+  if (rc) { m->d_blob.release(); delete m; return rc; }
   *out = m;
   return 0;
 }
-void mod_free(pai_mod* m) {
+// `wipe`: the modulus is part of a private key -- zero every buffer before it is freed, and the host copy of the modulus.
+// The coop constants are zeroed in any case.
+void mod_free(pai_mod* m, bool wipe) {
   if (!m) return;
   rt_set_device(m->device);
-  rt_free(m->d_blob);
-  rt_free(m->d_corr);
-  if (m->d_coop) { rt_memset(m->d_coop, 0, (size_t)3 * 32 * m->coopK * 4, 0); rt_sync(0); rt_free(m->d_coop); }
-  m->ws.release(); m->tmp_a.release(); m->tmp_b.release(); m->tmp_o.release(); m->tmp_s.release(); m->tmp_e.release();
+  m->d_blob.release(wipe);
+  m->d_corr.release(wipe);
+  m->d_coop.release(true);
+  m->ws.release(wipe);
+  for (DevBuf<>* b : {&m->tmp_a, &m->tmp_b, &m->tmp_o, &m->tmp_s, &m->tmp_e}) b->release(wipe);
+  if (wipe) std::fill(m->h_N.begin(), m->h_N.end(), 0);
   delete m;
 }
 
@@ -635,18 +689,10 @@ int do_mulmod(pai_mod* m, const uint32_t* consts, int cq, const uint32_t* a, con
 template <int NT>
 int do_powmod(pai_mod* m, const uint32_t* base, int base_tiles, const uint32_t* d_exp, int exp_limbs, long exp_stride,
               int nwin_fixed, uint32_t* out, long batch, rt_stream s) {
-  typedef PowBody<NT, W_VAR> B;
-  Geom g;
-  int cq = mc_limbs(NT) / 4;
-  int rc = geometry<B>(m->device, NT, cq, 3, batch, g);
-  if (rc) return rc;
-  rc = m->ws.get(s).tbl.ensure(table_bytes(g, NT, W_VAR));
-  if (rc) return rc;
-  unsigned long long* ctr = nullptr;
-  rc = m->ws.get(s).ctr.take(s, &ctr);
-  if (rc) return rc;
-  B body{m->d_blob, cq, base, base_tiles, d_exp, exp_limbs, exp_stride, nwin_fixed, out, batch, (u4*)m->ws.get(s).tbl.p, ctr};
-  return rt_launch(body, g.grid, g.nthr, g.smem, s);
+  const Shape sh{NT, mc_limbs(NT) / 4, 3, 1 << W_VAR};
+  return launch_persistent<PowBody<NT, W_VAR>>(m->device, m->ws.get(s), sh, batch, s, [&](u4* tbl, unsigned long long* ctr) {
+    return PowBody<NT, W_VAR>{m->d_blob.p, sh.cq, base, base_tiles, d_exp, exp_limbs, exp_stride, nwin_fixed, out, batch, tbl, ctr};
+  });
 }
 
 // product of `batch` rows modulo N -> one canonical row (two launches: per-CTA partial products, then their product
@@ -659,26 +705,26 @@ int do_reduce_mul(pai_mod* m, const uint32_t* rows, long batch, uint32_t* out, r
   const int cq = mc_limbs(NT) / 4;
   int rc = geometry<B>(m->device, NT, cq, 3, batch, g);
   if (rc) return rc;
-  if (!m->d_corr) {                                   // per-modulus table R^(2^i + 1), built on first use
-    rc = rt_malloc((void**)&m->d_corr, (size_t)REDUCE_CORR_ROWS * m->L * 4);
+  if (!m->d_corr.p) {                                 // per-modulus table R^(2^i + 1), built on first use
+    rc = m->d_corr.ensure((size_t)REDUCE_CORR_ROWS * m->L * 4);
     if (rc) return rc;
-    ReduceCorrBody<NT> cb{m->d_blob, cq, m->d_corr, REDUCE_CORR_ROWS};
+    ReduceCorrBody<NT> cb{m->d_blob.p, cq, m->d_corr.p, REDUCE_CORR_ROWS};
     rc = rt_launch(cb, 1, g.nthr, g.smem, s);
     if (!rc) rc = rt_sync(s);
-    if (rc) { rt_free(m->d_corr); m->d_corr = nullptr; return rc; }
+    if (rc) { m->d_corr.release(); return rc; }
   }
   const unsigned long long bits = (unsigned long long)batch;
   if (g.grid == 1) {
-    B body{m->d_blob, cq, rows, batch, out, m->d_corr, bits, 1};
+    B body{m->d_blob.p, cq, rows, batch, out, m->d_corr.p, bits, 1};
     return rt_launch(body, 1, g.nthr, g.smem, s);
   }
   StreamWs& w = m->ws.get(s);
   rc = w.red_a.ensure((size_t)g.grid * m->L * 4);
   if (rc) return rc;
-  B first{m->d_blob, cq, rows, batch, (uint32_t*)w.red_a.p, m->d_corr, 0ull, 0};
+  B first{m->d_blob.p, cq, rows, batch, (uint32_t*)w.red_a.p, m->d_corr.p, 0ull, 0};
   rc = rt_launch(first, g.grid, g.nthr, g.smem, s);
   if (rc) return rc;
-  B second{m->d_blob, cq, (const uint32_t*)w.red_a.p, (long)g.grid, out, m->d_corr, bits, 1};
+  B second{m->d_blob.p, cq, (const uint32_t*)w.red_a.p, (long)g.grid, out, m->d_corr.p, bits, 1};
   return rt_launch(second, 1, g.nthr, g.smem, s);
 }
 
@@ -689,7 +735,7 @@ int do_invert(pai_mod* m, const uint32_t* a, int a_tiles, const int32_t* flags, 
   int cq = mc_limbs(NT) / 4;
   int rc = geometry<B>(m->device, NT, cq, 4, batch, g);
   if (rc) return rc;
-  B body{m->d_blob, cq, a, a_tiles, flags, out, status, batch};
+  B body{m->d_blob.p, cq, a, a_tiles, flags, out, status, batch};
   return rt_launch(body, g.grid, g.nthr, g.smem, s);
 }
 
@@ -707,54 +753,35 @@ int do_invert_flagged(pai_mod* m, const uint32_t* a, const int32_t* flags, uint3
   if (seg > 32) seg = 32;
   const long nseg = (batch + seg - 1) / seg;
   g.grid = (int)std::max(1L, std::min((long)g.grid, (nseg + g.nthr - 1) / g.nthr));
-  B body{m->d_blob, cq, a, flags, out, status, batch, (int)seg};
+  B body{m->d_blob.p, cq, a, flags, out, status, batch, (int)seg};
   return rt_launch(body, g.grid, g.nthr, g.smem, s);
 }
 
 template <int NT>
+Shape enc_shape(const pai_pub* k) { return {NT, mc_limbs(NT) / 4 + NT, 2, k->nodd + 1}; }
+template <int NT>
 int do_encrypt(pai_pub* k, const uint32_t* m_, const uint32_t* r, uint32_t* c, long batch, rt_stream s) {
-  typedef EncBody<NT> B;
   pai_mod* m = k->nsq;
-  Geom g;
-  int cq = mc_limbs(NT) / 4 + NT;
-  int rc = geometry<B>(m->device, NT, cq, 2, batch, g);
-  if (rc) return rc;
-  rc = m->ws.get(s).tbl.ensure((size_t)g.grid * (size_t)(k->nodd + 1) * 2 * NT * g.nthr * 16);
-  if (rc) return rc;
-  unsigned long long* ctr = nullptr;
-  rc = m->ws.get(s).ctr.take(s, &ctr);
-  if (rc) return rc;
-  B body{m->d_blob, cq, k->d_prog, k->nops, k->nodd, m_, r, c, batch, (u4*)m->ws.get(s).tbl.p, ctr};
-  return rt_launch(body, g.grid, g.nthr, g.smem, s);
+  const Shape sh = enc_shape<NT>(k);
+  return launch_persistent<EncBody<NT>>(m->device, m->ws.get(s), sh, batch, s, [&](u4* tbl, unsigned long long* ctr) {
+    return EncBody<NT>{m->d_blob.p, sh.cq, k->d_prog, k->nops, k->nodd, m_, r, c, batch, tbl, ctr};
+  });
 }
 
 template <int NTH>
 int do_digit_setup(pai_mod* m, rt_stream s) {
-  void* scratch = nullptr;
-  int rc = rt_malloc(&scratch, (size_t)4 * 8 * NTH * 4);
-  if (rc) return rc;
-  DigitSetupBody<NTH> b{nullptr, 0, m->d_blob, (uint32_t*)scratch};
-  rc = rt_launch(b, 1, 32, 0, s);
-  if (!rc) rc = rt_sync(s);
-  rt_free(scratch);
-  return rc;
+  return run_setup((size_t)4 * 8 * NTH * 4, s, [&](uint32_t* scratch) { return DigitSetupBody<NTH>{nullptr, 0, m->d_blob.p, scratch}; });
 }
 
 template <int NTH>
+Shape enc_digit_shape(const pai_pub* k) { return {2 * NTH, dc_enc_limbs(NTH) / 4, 2, k->nodd + 1}; }
+template <int NTH>
 int do_encrypt_digit(pai_pub* k, const uint32_t* m_, const uint32_t* r, uint32_t* c, long batch, rt_stream s) {
-  typedef EncDigitBody<NTH> B;
   pai_mod* m = k->nmod;
-  Geom g;
-  int cq = dc_enc_limbs(NTH) / 4;
-  int rc = geometry<B>(m->device, 2 * NTH, cq, 2, batch, g);
-  if (rc) return rc;
-  rc = m->ws.get(s).tbl.ensure((size_t)g.grid * (size_t)(k->nodd + 1) * 4 * NTH * g.nthr * 16);
-  if (rc) return rc;
-  unsigned long long* ctr = nullptr;
-  rc = m->ws.get(s).ctr.take(s, &ctr);
-  if (rc) return rc;
-  B body{k->d_enc_consts, cq, k->d_prog, k->nops, k->nodd, m_, r, c, batch, (u4*)m->ws.get(s).tbl.p, ctr, m->d_blob + dc_zero_offset(NTH)};
-  return rt_launch(body, g.grid, g.nthr, g.smem, s);
+  const Shape sh = enc_digit_shape<NTH>(k);
+  return launch_persistent<EncDigitBody<NTH>>(m->device, m->ws.get(s), sh, batch, s, [&](u4* tbl, unsigned long long* ctr) {
+    return EncDigitBody<NTH>{k->d_enc_consts, sh.cq, k->d_prog, k->nops, k->nodd, m_, r, c, batch, tbl, ctr, m->d_blob.p + dc_zero_offset(NTH)};
+  });
 }
 
 // launch geometry of a tensor-core kernel: as many 128-thread groups per CTA as the body's register budget
@@ -795,30 +822,42 @@ int tc_geometry_of(int device, SmemFn smem_bytes, long batch, Geom& g) {
   return PAI_E_CUDA;
 #endif
 }
-template <int NTH>
-int tc_geometry(pai_pub* k, long batch, Geom& g) {
-  return tc_geometry_of<TcEncBody<NTH>, NTH>(k->nmod->device, [](int nthr) { return tc_enc_smem_bytes<NTH>(nthr); }, batch, g);
+// The tensor-core kernels run whole waves in one launch and a tail of less than a wave in a second launch with a
+// geometry of its own (tc_geometry_of).  launch(off, rows) runs rows [off, off + rows).
+template <class Launch>
+int tc_split(long wave, long batch, Launch launch) {
+  if (batch <= wave || batch % wave == 0) return launch(0L, batch);
+  const long head = batch - batch % wave;
+  int rc = launch(0L, head);
+  return rc ? rc : launch(head, batch - head);
+}
+// geometry (tc_geometry_of), the window-table workspace and the launch of a tensor-core kernel B over `batch` rows, with
+// `entries` table entries of 4 * NTH quads per thread; make(tbl) builds the body
+template <class B, int NTH, class SmemFn, class Make>
+int launch_tc(int device, StreamWs& w, SmemFn smem_bytes, long entries, long batch, rt_stream s, Make make) {
+  Geom g;
+  int rc = tc_geometry_of<B, NTH>(device, smem_bytes, batch, g);
+  if (!rc) rc = w.tbl.ensure((size_t)g.grid * entries * 4 * NTH * g.nthr * 16);
+  if (rc) return rc;
+  return rt_launch_group(make((u4*)w.tbl.p), g.grid, g.nthr, g.smem, s);
+}
+// rows one full grid of the tensor-core kernel B holds (0 when B cannot be resident)
+template <class B, int NTH>
+long tc_wave(int device, size_t (*smem_bytes)(int)) {
+  Geom g;
+  return tc_geometry_of<B, NTH>(device, smem_bytes, 1L << 40, g) ? 0 : wave_rows(g);
 }
 template <int NTH>
 int do_encrypt_tc(pai_pub* k, const uint32_t* m_, const uint32_t* r, uint32_t* c, long batch, rt_stream s) {
   typedef TcEncBody<NTH> B;
   pai_mod* m = k->nmod;
   Geom g;
-  int rc = tc_geometry<NTH>(k, 1L << 40, g);
-  if (rc) return rc;
-  const long wave = (long)g.grid * g.nthr;
-  if (batch > wave && batch % wave) {               // whole waves, then the tail with a geometry of its own (tc_geometry_of)
-    const long head = batch - batch % wave;
-    rc = do_encrypt_tc<NTH>(k, m_, r, c, head, s);
-    if (rc) return rc;
-    return do_encrypt_tc<NTH>(k, m_ + head * 8 * NTH, r + head * 8 * NTH, c + head * 16 * NTH, batch - head, s);
-  }
-  rc = tc_geometry<NTH>(k, batch, g);
+  int rc = tc_geometry_of<B, NTH>(m->device, tc_enc_smem_bytes<NTH>, batch, g);
   if (rc) return rc;
   rc = m->ws.get(s).tbl.ensure((size_t)g.grid * (size_t)(k->nodd + 4) * 4 * NTH * g.nthr * 16);
   if (rc) return rc;
   B body{k->d_enc_consts, dc_enc_limbs(NTH) / 4, k->d_prog, k->nops, k->nodd, m_, r, c, batch, (u4*)m->ws.get(s).tbl.p,
-         m->d_blob + dc_zero_offset(NTH), k->d_tc, k->tc_stagger, nullptr};
+         m->d_blob.p + dc_zero_offset(NTH), k->d_tc, k->tc_stagger, nullptr};
 #if !defined(PAI_HOSTSIM)
   // development aid: PAI_TC_PROF=<file> dumps per-warp cycle counters of the phases of tc_op after a synchronous launch
   if (const char* pf = getenv("PAI_TC_PROF")) {
@@ -845,14 +884,9 @@ template <int NTH>
 int do_powmod_tc(pai_pub* k, const uint32_t* base, const uint32_t* d_exp, int exp_limbs, uint32_t* out, long batch, rt_stream s) {
   typedef TcPowBody<NTH, W_VAR> B;
   pai_mod* m = k->nmod;
-  Geom g;
-  int rc = tc_geometry_of<B, NTH>(m->device, [](int nthr) { return tc_pow_smem_bytes<NTH>(nthr); }, batch, g);
-  if (rc) return rc;
-  rc = m->ws.get(s).tbl.ensure((size_t)g.grid * (((size_t)1 << W_VAR) + 3) * 4 * NTH * g.nthr * 16);
-  if (rc) return rc;
-  B body{k->d_enc_consts, dc_pow_limbs(NTH) / 4, base, d_exp, exp_limbs, out, batch, (u4*)m->ws.get(s).tbl.p,
-         m->d_blob + dc_zero_offset(NTH), k->d_tc, k->tc_stagger};
-  return rt_launch_group(body, g.grid, g.nthr, g.smem, s);
+  return launch_tc<B, NTH>(m->device, m->ws.get(s), tc_pow_smem_bytes<NTH>, (1 << W_VAR) + 3, batch, s, [&](u4* tbl) {
+    return B{k->d_enc_consts, dc_pow_limbs(NTH) / 4, base, d_exp, exp_limbs, out, batch, tbl, m->d_blob.p + dc_zero_offset(NTH), k->d_tc, k->tc_stagger};
+  });
 }
 // Straus groups: one thread per group of gsz elements; gsz is chosen so that the groups fill about one wave
 template <int NTH>
@@ -861,66 +895,32 @@ int do_straus_tc(pai_pub* k, const uint32_t* base, const uint32_t* d_exp, int ex
   typedef TcStrausBody<NTH, W_VAR> B;
   pai_mod* m = k->nmod;
   Geom g;
-  int rc = tc_geometry_of<B, NTH>(m->device, [](int nthr) { return tc_pow_smem_bytes<NTH>(nthr); }, 1L << 40, g);
+  int rc = tc_geometry_of<B, NTH>(m->device, tc_pow_smem_bytes<NTH>, 1L << 40, g);
   if (rc) return rc;
   const long wave = (long)g.grid * g.nthr;
   long gsz = (batch + wave - 1) / wave;
   if (gsz < 1) gsz = 1;
   if (gsz > 32) gsz = 32;
   const long ngroups = (batch + gsz - 1) / gsz;
-  rc = tc_geometry_of<B, NTH>(m->device, [](int nthr) { return tc_pow_smem_bytes<NTH>(nthr); }, ngroups, g);
-  if (rc) return rc;
-  rc = m->ws.get(s).tbl.ensure((size_t)g.grid * (((size_t)gsz << W_VAR) + 4) * 4 * NTH * g.nthr * 16);
-  if (rc) return rc;
-  B body{k->d_enc_consts, dc_pow_limbs(NTH) / 4, base, d_exp, exp_limbs, (int)gsz, partial, batch, (u4*)m->ws.get(s).tbl.p,
-         m->d_blob + dc_zero_offset(NTH), k->d_tc, k->tc_stagger};
   *ngroups_out = ngroups;
-  return rt_launch_group(body, g.grid, g.nthr, g.smem, s);
-}
-template <int NTH>
-long encrypt_wave_tc(pai_pub* k) {
-  Geom g;
-  if (tc_geometry<NTH>(k, 1L << 40, g)) return 0;
-  return (long)g.grid * g.nthr;
+  return launch_tc<B, NTH>(m->device, m->ws.get(s), tc_pow_smem_bytes<NTH>, (gsz << W_VAR) + 4, ngroups, s, [&](u4* tbl) {
+    return B{k->d_enc_consts, dc_pow_limbs(NTH) / 4, base, d_exp, exp_limbs, (int)gsz, partial, batch, tbl, m->d_blob.p + dc_zero_offset(NTH), k->d_tc, k->tc_stagger};
+  });
 }
 template <int NTH>
 int do_tc_setup(pai_pub* k, rt_stream s) {
-  void* scratch = nullptr;
-  int rc = rt_malloc(&scratch, (size_t)8 * NTH * 4);
-  if (!rc) rc = rt_malloc((void**)&k->d_tc, (size_t)tc_blob_bytes(NTH));
-  if (!rc) {
-    TcSetupBody<NTH> b{nullptr, 0, k->nmod->d_blob, k->d_tc, (uint32_t*)scratch};
-    rc = rt_launch(b, 1, 32, 0, s);
-  }
-  if (!rc) rc = rt_sync(s);
-  rt_free(scratch);
-  return rc;
+  int rc = rt_malloc((void**)&k->d_tc, (size_t)tc_blob_bytes(NTH));
+  if (rc) return rc;
+  return run_setup((size_t)8 * NTH * 4, s, [&](uint32_t* scratch) { return TcSetupBody<NTH>{nullptr, 0, k->nmod->d_blob.p, k->d_tc, scratch}; });
 }
-
-template <class B>
-long wave_of(int device, int NT, int cq, int nbuf) {
-  Geom g;
-  if (geometry<B>(device, NT, cq, nbuf, 1L << 40, g)) return 0;
-  return (long)g.grid * g.nthr;
-}
-template <int NTH>
-long encrypt_wave_digit(pai_pub* k) { return wave_of<EncDigitBody<NTH>>(k->nmod->device, 2 * NTH, dc_enc_limbs(NTH) / 4, 2); }
 
 template <int NTH>
 int do_powmod_digit(pai_pub* k, const uint32_t* base, const uint32_t* d_exp, int exp_limbs, uint32_t* out, long batch, rt_stream s) {
-  typedef PowDigitBody<NTH, W_VAR> B;
   pai_mod* m = k->nmod;
-  Geom g;
-  int cq = dc_pow_limbs(NTH) / 4;
-  int rc = geometry<B>(m->device, 2 * NTH, cq, 2, batch, g);
-  if (rc) return rc;
-  rc = m->ws.get(s).tbl.ensure((size_t)g.grid * ((size_t)1 << W_VAR) * 4 * NTH * g.nthr * 16);
-  if (rc) return rc;
-  unsigned long long* ctr = nullptr;
-  rc = m->ws.get(s).ctr.take(s, &ctr);
-  if (rc) return rc;
-  B body{k->d_enc_consts, cq, base, d_exp, exp_limbs, out, batch, (u4*)m->ws.get(s).tbl.p, ctr, m->d_blob + dc_zero_offset(NTH)};
-  return rt_launch(body, g.grid, g.nthr, g.smem, s);
+  const Shape sh{2 * NTH, dc_pow_limbs(NTH) / 4, 2, 1 << W_VAR};
+  return launch_persistent<PowDigitBody<NTH, W_VAR>>(m->device, m->ws.get(s), sh, batch, s, [&](u4* tbl, unsigned long long* ctr) {
+    return PowDigitBody<NTH, W_VAR>{k->d_enc_consts, sh.cq, base, d_exp, exp_limbs, out, batch, tbl, ctr, m->d_blob.p + dc_zero_offset(NTH)};
+  });
 }
 
 // Window width of the matrix-vector product: the w in 1..8 with the fewest modular multiplications,
@@ -950,7 +950,7 @@ int do_matvec_digit(pai_pub* k, StreamWs& w, const uint32_t* c, const uint32_t* 
                     const uint8_t* neg, long nnz, long nrows, uint32_t* out, rt_stream s) {
   pai_mod* m = k->nmod;
   const int cq = dc_pow_limbs(NTH) / 4;
-  const uint32_t* gzero = m->d_blob + dc_zero_offset(NTH);
+  const uint32_t* gzero = m->d_blob.p + dc_zero_offset(NTH);
   int rc = 0;
   if (nnz > 0) {
     typedef MatTblBody<NTH> TB;
@@ -962,93 +962,54 @@ int do_matvec_digit(pai_pub* k, StreamWs& w, const uint32_t* c, const uint32_t* 
     rc = rt_launch(tb, g.grid, g.nthr, g.smem, s);
     if (rc) return rc;
   }
-  typedef MatRowBody<NTH> RB;
-  Geom g;
-  rc = geometry<RB>(m->device, 2 * NTH, cq, 2, nrows, g);
-  if (rc) return rc;
-  unsigned long long* ctr = nullptr;
-  rc = w.ctr.take(s, &ctr);
-  if (rc) return rc;
-  RB rb{k->d_enc_consts, cq, (const u4*)w.mv_tbl.p, ncols, win, indptr, indices, mag, ml, neg, out, nrows, ctr, gzero};
-  return rt_launch(rb, g.grid, g.nthr, g.smem, s);
+  return launch_persistent<MatRowBody<NTH>>(m->device, w, {2 * NTH, cq, 2, 0}, nrows, s, [&](u4*, unsigned long long* ctr) {
+    return MatRowBody<NTH>{k->d_enc_consts, cq, (const u4*)w.mv_tbl.p, ncols, win, indptr, indices, mag, ml, neg, out, nrows, ctr, gzero};
+  });
 }
 
+// constant quads of one CRT side of the full-width decrypt: [ blob(x^2) | blob(x) | xinv | hM | e ]
+int side_quads_of(int NTP) { return mc_limbs(2 * NTP) / 4 + mc_limbs(NTP) / 4 + 6 * NTP; }
+// constant quads of the digit and tensor-core decrypt: [ P: dblob(p) | hM | e ][ Q: ... ][ pinvqM ]
+template <int NTP>
+int dconst_quads() { return 2 * (dside_limbs<NTP>() / 4) + 2 * NTP; }
+
+template <int NTP>
+Shape dec_shape() { return {2 * NTP, 2 * side_quads_of(NTP) + 2 * NTP, 3, 1 << W_DEC}; }
 template <int NTP>
 int do_decrypt(pai_priv* k, const uint32_t* c, uint32_t* out, long batch, rt_stream s, const uint32_t* pre_p = nullptr,
                const uint32_t* pre_q = nullptr) {
-  typedef DecBody<NTP, W_DEC> B;
-  Geom g;
-  int cq = 2 * (mc_limbs(2 * NTP) / 4 + mc_limbs(NTP) / 4 + 6 * NTP) + 2 * NTP;
-  int rc = geometry<B>(k->device, 2 * NTP, cq, 3, batch, g);
-  if (rc) return rc;
-  rc = k->ws.get(s).tbl.ensure(table_bytes(g, 2 * NTP, W_DEC));
-  if (rc) return rc;
-  unsigned long long* ctr = nullptr;
-  rc = k->ws.get(s).ctr.take(s, &ctr);
-  if (rc) return rc;
-  B body{k->d_consts, cq, k->nwin_p, k->nwin_q, c, out, batch, (u4*)k->ws.get(s).tbl.p, ctr, pre_p, pre_q};
-  return rt_launch(body, g.grid, g.nthr, g.smem, s);
+  const Shape sh = dec_shape<NTP>();
+  return launch_persistent<DecBody<NTP, W_DEC>>(k->device, k->ws.get(s), sh, batch, s, [&](u4* tbl, unsigned long long* ctr) {
+    return DecBody<NTP, W_DEC>{k->d_consts.p, sh.cq, k->nwin_p, k->nwin_q, c, out, batch, tbl, ctr, pre_p, pre_q};
+  });
 }
 
+template <int NTP>
+Shape dec_digit_shape() { return {2 * NTP, dconst_quads<NTP>(), 2, 1 << W_DEC}; }
 template <int NTP>
 int do_decrypt_digit(pai_priv* k, const uint32_t* c, uint32_t* out, long batch, rt_stream s) {
-  typedef DecDigitBody<NTP, W_DEC> B;
-  Geom g;
-  int cq = 2 * (dside_limbs<NTP>() / 4) + 2 * NTP;
-  int rc = geometry<B>(k->device, 2 * NTP, cq, 2, batch, g);
-  if (rc) return rc;
-  rc = k->ws.get(s).tbl.ensure((size_t)g.grid * ((size_t)1 << W_DEC) * 4 * NTP * g.nthr * 16);
-  if (rc) return rc;
-  unsigned long long* ctr = nullptr;
-  rc = k->ws.get(s).ctr.take(s, &ctr);
-  if (rc) return rc;
-  B body{k->d_dconsts, cq, k->nwin_p, k->nwin_q, c, out, batch, (u4*)k->ws.get(s).tbl.p, ctr};
-  return rt_launch(body, g.grid, g.nthr, g.smem, s);
+  const Shape sh = dec_digit_shape<NTP>();
+  return launch_persistent<DecDigitBody<NTP, W_DEC>>(k->device, k->ws.get(s), sh, batch, s, [&](u4* tbl, unsigned long long* ctr) {
+    return DecDigitBody<NTP, W_DEC>{k->d_dconsts.p, sh.cq, k->nwin_p, k->nwin_q, c, out, batch, tbl, ctr};
+  });
 }
 
-template <int NTP>
-int tc_dec_geometry(pai_priv* k, long batch, Geom& g) {
-  return tc_geometry_of<TcDecBody<NTP, W_DEC>, NTP>(k->device, [](int nthr) { return tc_dec_smem_bytes<NTP>(nthr); }, batch, g);
-}
 template <int NTP>
 int do_decrypt_tc(pai_priv* k, const uint32_t* c, uint32_t* out, long batch, rt_stream s) {
   typedef TcDecBody<NTP, W_DEC> B;
-  Geom g;
-  int rc = tc_dec_geometry<NTP>(k, 1L << 40, g);
-  if (rc) return rc;
-  const long wave = (long)g.grid * g.nthr;
-  if (batch > wave && batch % wave) {               // whole waves, then the tail with a geometry of its own (tc_geometry_of)
-    const long head = batch - batch % wave;
-    rc = do_decrypt_tc<NTP>(k, c, out, head, s);
-    if (rc) return rc;
-    return do_decrypt_tc<NTP>(k, c + head * 32 * NTP, out + head * 16 * NTP, batch - head, s);
-  }
-  rc = tc_dec_geometry<NTP>(k, batch, g);
-  if (rc) return rc;
-  rc = k->ws.get(s).tbl.ensure((size_t)g.grid * (((size_t)1 << W_DEC) + 3) * 4 * NTP * g.nthr * 16);
-  if (rc) return rc;
-  int cq = 2 * (dside_limbs<NTP>() / 4) + 2 * NTP;
-  B body{k->d_dconsts, cq, k->nwin_p, k->nwin_q, c, out, batch, (u4*)k->ws.get(s).tbl.p, k->d_tc, k->tc_stagger};
-  return rt_launch_group(body, g.grid, g.nthr, g.smem, s);
-}
-template <int NTP>
-long decrypt_wave_tc(pai_priv* k) {
-  Geom g;
-  if (tc_dec_geometry<NTP>(k, 1L << 40, g)) return 0;
-  return (long)g.grid * g.nthr;
+  return launch_tc<B, NTP>(k->device, k->ws.get(s), tc_dec_smem_bytes<NTP>, (1 << W_DEC) + 3, batch, s, [&](u4* tbl) {
+    return B{k->d_dconsts.p, dconst_quads<NTP>(), k->nwin_p, k->nwin_q, c, out, batch, tbl, k->d_tc.p, k->tc_stagger};
+  });
 }
 template <int NTP>
 int do_priv_tc_setup(pai_priv* k, rt_stream s) {
-  void* scratch = nullptr;
-  int rc = rt_malloc(&scratch, (size_t)8 * NTP * 4);
-  if (!rc) rc = rt_malloc((void**)&k->d_tc, (size_t)2 * tc_blob_bytes(NTP));
+  int rc = k->d_tc.ensure((size_t)2 * tc_blob_bytes(NTP));
   pai_mod* md[2] = {k->pd, k->qd};
   for (int i = 0; i < 2 && !rc; i++) {
-    TcSetupBody<NTP> b{nullptr, 0, md[i]->d_blob, k->d_tc + (size_t)i * tc_blob_bytes(NTP), (uint32_t*)scratch};
-    rc = rt_launch(b, 1, 32, 0, s);
-    if (!rc) rc = rt_sync(s);
+    rc = run_setup((size_t)8 * NTP * 4, s, [&](uint32_t* scratch) {
+      return TcSetupBody<NTP>{nullptr, 0, md[i]->d_blob.p, k->d_tc.p + (size_t)i * tc_blob_bytes(NTP), scratch};
+    });
   }
-  rt_free(scratch);
   return rc;
 }
 
@@ -1059,31 +1020,21 @@ int do_priv_digit_setup(pai_priv* k, rt_stream s) {
   const int L1 = 8 * NTP;
   int rc = mod_create_impl(k->h_p.data(), L1, k->device, NTP, dc_extra_limbs(NTP), &k->pd);
   if (!rc) rc = mod_create_impl(k->h_q.data(), L1, k->device, NTP, dc_extra_limbs(NTP), &k->qd);
+  if (!rc) rc = do_digit_setup<NTP>(k->pd, s);
+  if (!rc) rc = do_digit_setup<NTP>(k->qd, s);
+  if (!rc) rc = k->d_dconsts.ensure((size_t)dconst_quads<NTP>() * 16);
   if (rc) return rc;
-  for (pai_mod* m : {k->pd, k->qd}) {
-    void* scratch = nullptr;
-    rc = rt_malloc(&scratch, (size_t)4 * L1 * 4);
-    if (rc) return rc;
-    DigitSetupBody<NTP> b{nullptr, 0, m->d_blob, (uint32_t*)scratch};
-    rc = rt_launch(b, 1, 32, 0, s);
-    if (!rc) rc = rt_sync(s);
-    rt_free(scratch);
-    if (rc) return rc;
-  }
   const int side = dside_limbs<NTP>();
-  size_t total = ((size_t)2 * side + L1) * 4;
-  rc = rt_malloc((void**)&k->d_dconsts, total);
-  if (rc) return rc;
-  const int old_side = mc_limbs(2 * NTP) + mc_limbs(NTP) + 3 * L1;     // [ blob(x^2) | blob(x) | xinv | hM | e ]
+  const int old_side = 4 * side_quads_of(NTP);                          // [ blob(x^2) | blob(x) | xinv | hM | e ]
   const int old_hM = mc_limbs(2 * NTP) + mc_limbs(NTP) + L1;
   pai_mod* md[2] = {k->pd, k->qd};
   for (int i = 0; i < 2 && !rc; i++) {
-    uint32_t* dst = k->d_dconsts + (size_t)i * side;
-    const uint32_t* old = k->d_consts + (size_t)i * old_side;
-    rc = rt_d2d(dst, md[i]->d_blob, (size_t)dc_limbs(NTP) * 4, s);
+    uint32_t* dst = k->d_dconsts.p + (size_t)i * side;
+    const uint32_t* old = k->d_consts.p + (size_t)i * old_side;
+    rc = rt_d2d(dst, md[i]->d_blob.p, (size_t)dc_limbs(NTP) * 4, s);
     if (!rc) rc = rt_d2d(dst + dc_limbs(NTP), old + old_hM, (size_t)2 * L1 * 4, s);      // hM | e
   }
-  if (!rc) rc = rt_d2d(k->d_dconsts + (size_t)2 * side, k->d_consts + (size_t)2 * old_side, (size_t)L1 * 4, s);   // pinvqM
+  if (!rc) rc = rt_d2d(k->d_dconsts.p + (size_t)2 * side, k->d_consts.p + (size_t)2 * old_side, (size_t)L1 * 4, s);   // pinvqM
   if (!rc) rc = rt_sync(s);
   return rc;
 }
@@ -1098,8 +1049,8 @@ int do_side(pai_priv* k, pai_mod* m2, pai_mod* m1, const limbs_t& x, const limbs
   uint32_t* d_xinv = d_b1 + mc_limbs(NTP);
   uint32_t* d_hM = d_xinv + L1;
   uint32_t* d_e = d_hM + L1;
-  int rc = rt_d2d(d_b2, m2->d_blob, (size_t)mc_limbs(NT2) * 4, s);
-  if (!rc) rc = rt_d2d(d_b1, m1->d_blob, (size_t)mc_limbs(NTP) * 4, s);
+  int rc = rt_d2d(d_b2, m2->d_blob.p, (size_t)mc_limbs(NT2) * 4, s);
+  if (!rc) rc = rt_d2d(d_b1, m1->d_blob.p, (size_t)mc_limbs(NTP) * 4, s);
   // x^-1 mod 2^(256 NTP)
   if (!rc) { XinvBody xb{nullptr, 0, d_xinv, d_b1 /* N of blob(x) */, L1}; rc = rt_launch(xb, 1, 32, 0, s); }
   // exponent x - 1
@@ -1109,44 +1060,41 @@ int do_side(pai_priv* k, pai_mod* m2, pai_mod* m1, const limbs_t& x, const limbs
   if (!rc) rc = rt_d2d(d_hM, d_b1 + L1, (size_t)L1 * 4, s);
   if (rc) return rc;
   // l = L(g^(x-1) mod x^2) mod x  via one CRT half with h = 1 on the "ciphertext" g = n + 1
-  void *d_g = nullptr, *d_l = nullptr, *d_h = nullptr, *d_st = nullptr, *d_hm = nullptr;
-  rc = rt_malloc(&d_g, (size_t)2 * 8 * NT2 * 4);
-  if (!rc) rc = rt_malloc(&d_l, (size_t)L1 * 4);
-  if (!rc) rc = rt_malloc(&d_h, (size_t)L1 * 4);
-  if (!rc) rc = rt_malloc(&d_hm, (size_t)L1 * 4);
-  if (!rc) rc = rt_malloc(&d_st, 16);
-  if (!rc) rc = rt_h2d(d_g, g_pad.data(), (size_t)2 * 8 * NT2 * 4, s);
+  TmpBuf d_g, d_l, d_h, d_st, d_hm;
+  rc = d_g.alloc((size_t)2 * 8 * NT2 * 4);
+  if (!rc) rc = d_l.alloc((size_t)L1 * 4);
+  if (!rc) rc = d_h.alloc((size_t)L1 * 4);
+  if (!rc) rc = d_hm.alloc((size_t)L1 * 4);
+  if (!rc) rc = d_st.alloc(16);
+  if (!rc) rc = rt_h2d(d_g.p, g_pad.data(), (size_t)2 * 8 * NT2 * 4, s);
   if (!rc) {
     typedef LBody<NTP, W_DEC> B;
-    int cq = mc_limbs(NT2) / 4 + mc_limbs(NTP) / 4 + 6 * NTP;
+    const int cq = side_quads_of(NTP);
     Geom g;
     rc = geometry<B>(k->device, NT2, cq, 3, 1, g);
-    if (!rc) rc = k->ws.get(s).tbl.ensure(table_bytes(g, NT2, W_DEC));
-    if (!rc) { B body{d_side, cq, nwin, (const uint32_t*)d_g, (uint32_t*)d_l, (u4*)k->ws.get(s).tbl.p}; rc = rt_launch(body, 1, g.nthr, g.smem, s); }
+    if (!rc) rc = k->ws.get(s).tbl.ensure((size_t)g.grid * ((size_t)1 << W_DEC) * 2 * NT2 * g.nthr * 16);
+    if (!rc) { B body{d_side, cq, nwin, d_g.u32(), d_l.u32(), (u4*)k->ws.get(s).tbl.p}; rc = rt_launch(body, 1, g.nthr, g.smem, s); }
   }
   // h = l^-1 mod x  (phe/paillier.py:360), then hM = h * R mod x
-  if (!rc) rc = do_invert<NTP>(m1, (const uint32_t*)d_l, NTP, nullptr, (uint32_t*)d_h, (int32_t*)d_st, 1, s);
+  if (!rc) rc = do_invert<NTP>(m1, d_l.u32(), NTP, nullptr, d_h.u32(), (int32_t*)d_st.p, 1, s);
   int32_t st = 0;
-  if (!rc) rc = rt_d2h(&st, d_st, 4, s);
+  if (!rc) rc = rt_d2h(&st, d_st.p, 4, s);
   if (!rc) rc = rt_sync(s);
   if (!rc && st) { g_err = "h_function: inverse does not exist"; rc = PAI_E_NOINV; }
-  if (!rc) rc = do_mulmod<NTP>(m1, m1->d_blob, mc_limbs(NTP) / 4, (const uint32_t*)d_h, m1->d_blob + L1 /* R1 as a plain number */,
-                               (uint32_t*)d_hm, 1, s);
-  if (!rc) rc = rt_d2d(d_hM, d_hm, (size_t)L1 * 4, s);
+  if (!rc) rc = do_mulmod<NTP>(m1, m1->d_blob.p, mc_limbs(NTP) / 4, d_h.u32(), m1->d_blob.p + L1 /* R1 as a plain number */, d_hm.u32(), 1, s);
+  if (!rc) rc = rt_d2d(d_hM, d_hm.p, (size_t)L1 * 4, s);
   h_out.assign(L1, 0);
-  if (!rc) rc = rt_d2h(h_out.data(), d_h, (size_t)L1 * 4, s);
+  if (!rc) rc = rt_d2h(h_out.data(), d_h.p, (size_t)L1 * 4, s);
   if (!rc) rc = rt_sync(s);
-  rt_free(d_g); rt_free(d_l); rt_free(d_h); rt_free(d_hm); rt_free(d_st);
   return rc;
 }
 
 template <int NTP>
 int do_priv_setup(pai_priv* k, rt_stream s) {
   const int L1 = 8 * NTP, NT2 = 2 * NTP;
-  const int sideq = mc_limbs(NT2) / 4 + mc_limbs(NTP) / 4 + 6 * NTP;
-  size_t total = ((size_t)2 * sideq + 2 * NTP) * 16;
-  int rc = rt_malloc((void**)&k->d_consts, total);
-  if (!rc) rc = rt_memset(k->d_consts, 0, total, s);
+  const int sideq = side_quads_of(NTP);
+  int rc = k->d_consts.ensure(((size_t)2 * sideq + 2 * NTP) * 16);
+  if (!rc) rc = rt_memset(k->d_consts.p, 0, k->d_consts.bytes, s);
   if (rc) return rc;
   limbs_t p = padded(k->h_p.data(), L1, L1), q = padded(k->h_q.data(), L1, L1);
   limbs_t n = h_mul(p, q);                         // 2*L1 limbs
@@ -1154,30 +1102,29 @@ int do_priv_setup(pai_priv* k, rt_stream s) {
   limbs_t g_pad = padded(g.data(), (int)g.size(), 2 * 8 * NT2);
   k->nwin_p = (bit_length(h_sub_small(p, 1)) + W_DEC - 1) / W_DEC;
   k->nwin_q = (bit_length(h_sub_small(q, 1)) + W_DEC - 1) / W_DEC;
-  uint32_t* d_P = k->d_consts;
-  uint32_t* d_Q = k->d_consts + (size_t)sideq * 4;
-  uint32_t* d_pinvqM = k->d_consts + (size_t)2 * sideq * 4;
+  uint32_t* d_P = k->d_consts.p;
+  uint32_t* d_Q = k->d_consts.p + (size_t)sideq * 4;
+  uint32_t* d_pinvqM = k->d_consts.p + (size_t)2 * sideq * 4;
   rc = do_side<NTP>(k, k->p2, k->p1, p, g_pad, d_P, k->nwin_p, k->h_hp, s);
   if (!rc) rc = do_side<NTP>(k, k->q2, k->q1, q, g_pad, d_Q, k->nwin_q, k->h_hq, s);
   if (rc) return rc;
   // p_inverse = p^-1 mod q (phe/paillier.py:233); pinvqM = p_inverse * R mod q
-  void *d_p = nullptr, *d_pi = nullptr, *d_st = nullptr, *d_pm = nullptr;
-  rc = rt_malloc(&d_p, (size_t)L1 * 4);
-  if (!rc) rc = rt_malloc(&d_pi, (size_t)L1 * 4);
-  if (!rc) rc = rt_malloc(&d_pm, (size_t)L1 * 4);
-  if (!rc) rc = rt_malloc(&d_st, 16);
-  if (!rc) rc = rt_h2d(d_p, p.data(), (size_t)L1 * 4, s);
-  if (!rc) rc = do_invert<NTP>(k->q1, (const uint32_t*)d_p, NTP, nullptr, (uint32_t*)d_pi, (int32_t*)d_st, 1, s);
+  TmpBuf d_p, d_pi, d_st, d_pm;
+  rc = d_p.alloc((size_t)L1 * 4);
+  if (!rc) rc = d_pi.alloc((size_t)L1 * 4);
+  if (!rc) rc = d_pm.alloc((size_t)L1 * 4);
+  if (!rc) rc = d_st.alloc(16);
+  if (!rc) rc = rt_h2d(d_p.p, p.data(), (size_t)L1 * 4, s);
+  if (!rc) rc = do_invert<NTP>(k->q1, d_p.u32(), NTP, nullptr, d_pi.u32(), (int32_t*)d_st.p, 1, s);
   int32_t st = 0;
-  if (!rc) rc = rt_d2h(&st, d_st, 4, s);
+  if (!rc) rc = rt_d2h(&st, d_st.p, 4, s);
   if (!rc) rc = rt_sync(s);
   if (!rc && st) { g_err = "p has no inverse mod q"; rc = PAI_E_NOINV; }
-  if (!rc) rc = do_mulmod<NTP>(k->q1, k->q1->d_blob, mc_limbs(NTP) / 4, (const uint32_t*)d_pi, k->q1->d_blob + L1, (uint32_t*)d_pm, 1, s);
-  if (!rc) rc = rt_d2d(d_pinvqM, d_pm, (size_t)L1 * 4, s);
+  if (!rc) rc = do_mulmod<NTP>(k->q1, k->q1->d_blob.p, mc_limbs(NTP) / 4, d_pi.u32(), k->q1->d_blob.p + L1, d_pm.u32(), 1, s);
+  if (!rc) rc = rt_d2d(d_pinvqM, d_pm.p, (size_t)L1 * 4, s);
   k->h_pinv.assign(L1, 0);
-  if (!rc) rc = rt_d2h(k->h_pinv.data(), d_pi, (size_t)L1 * 4, s);
+  if (!rc) rc = rt_d2h(k->h_pinv.data(), d_pi.p, (size_t)L1 * 4, s);
   if (!rc) rc = rt_sync(s);
-  rt_free(d_p); rt_free(d_pi); rt_free(d_pm); rt_free(d_st);
   return rc;
 }
 
@@ -1207,23 +1154,23 @@ static long coop_rows(long batch, long wave) {
   const long tail = wave > 0 ? batch % wave : 0;
   return tail <= lim ? tail : 0;
 }
-static int coop_geometry(int device, int K, long items, int* grid, size_t* smem) {
-  *smem = (size_t)COOP_WARPS * (1 << COOP_W) * K * 32 * 4;
-  // one CTA (= one warp) per item, no grid-stride loop: the hardware block scheduler refills SMs as items finish
-  (void)device;
-  *grid = (int)std::min<long>((items + COOP_WARPS - 1) / COOP_WARPS, 1L << 30);
-  return 0;
+// one CTA (= one warp) per item, no grid-stride loop: the hardware block scheduler refills SMs as items finish
+template <int K, class B>
+static int launch_coop(const B& b, long items, rt_stream s) {
+  const int grid = (int)std::min<long>((items + COOP_WARPS - 1) / COOP_WARPS, 1L << 30);
+  return rt_launch_coop(b, grid, 32 * COOP_WARPS, (size_t)COOP_WARPS * (1 << COOP_W) * K * 32 * 4, s);
 }
 // constants of the modulus in the warp layout, computed once with the generic kernels: 2^(64 Lc) and 2^(96 Lc) mod N
 static int ensure_coop(pai_mod* m, rt_stream s) {
-  if (m->d_coop) return 0;
+  if (m->coopK) return 0;
   const int Lc = (m->L + 31) / 32 * 32, K = Lc / 32;
   if (K != 1 && K != 2 && K != 3 && K != 4 && K != 6 && K != 8) { g_err = "unsupported operand size"; return PAI_E_ARG; }
-  uint32_t* blob = nullptr;
-  uint32_t* tmp = nullptr;
-  int rc = rt_malloc((void**)&blob, (size_t)3 * Lc * 4);
-  if (!rc) rc = rt_malloc((void**)&tmp, (size_t)2 * m->L * 4);
-  if (!rc) rc = rt_memset(blob, 0, (size_t)3 * Lc * 4, s);
+  TmpBuf tmp_buf;
+  int rc = m->d_coop.ensure((size_t)3 * Lc * 4);
+  if (!rc) rc = tmp_buf.alloc((size_t)2 * m->L * 4);
+  uint32_t* blob = m->d_coop.p;
+  uint32_t* tmp = tmp_buf.u32();
+  if (!rc) rc = rt_memset(blob, 0, m->d_coop.bytes, s);
   if (!rc) rc = rt_h2d(blob, m->h_N.data(), (size_t)m->L * 4, s);
   limbs_t two(m->L, 0);
   two[0] = 2;
@@ -1236,13 +1183,11 @@ static int ensure_coop(pai_mod* m, rt_stream s) {
   }
   m->coop_building = false;
   if (!rc) rc = rt_sync(s);
-  rt_free(tmp);
-  if (rc) { rt_free(blob); return rc; }
+  if (rc) { m->d_coop.release(); return rc; }
   uint32_t n0 = m->h_N[0], i0 = n0;
   for (int i = 0; i < 5; i++) i0 *= 2u - n0 * i0;
   m->coop_n0inv = 0u - i0;                       // -N^-1 mod 2^32
   m->coopK = K;
-  m->d_coop = blob;
   return 0;
 }
 template <int K>
@@ -1250,36 +1195,30 @@ static int do_coop_powmod(pai_mod* m, const uint32_t* d_base, int base_limbs, co
                           uint32_t* d_out, long batch, rt_stream s) {
   CoopPowBody<K> b;
   b.consts = nullptr; b.const_quads = 0; b.nsides = 1;
-  b.blob[0] = b.blob[1] = m->d_coop; b.n0inv[0] = b.n0inv[1] = m->coop_n0inv;
+  b.blob[0] = b.blob[1] = m->d_coop.p; b.n0inv[0] = b.n0inv[1] = m->coop_n0inv;
   b.e[0] = b.e[1] = d_exp; b.e_limbs = exp_limbs; b.nwin[0] = b.nwin[1] = (nbits + COOP_W - 1) / COOP_W;
   b.out[0] = b.out[1] = d_out; b.base = d_base; b.base_limbs = base_limbs; b.out_limbs = m->L; b.batch = batch;
-  int grid; size_t smem;
-  coop_geometry(m->device, K, batch, &grid, &smem);
-  return rt_launch_coop(b, grid, 32 * COOP_WARPS, smem, s);
+  return launch_coop<K>(b, batch, s);
 }
 
 template <int K>
 static int do_coop_encrypt(pai_pub* k, const uint32_t* d_m, const uint32_t* d_r, uint32_t* d_c, long batch, rt_stream s) {
   pai_mod* m = k->nsq;
   const int nwin = (bit_length(k->h_n) + COOP_W - 1) / COOP_W;
-  CoopEncBody<K> b{nullptr, 0, m->d_coop, m->coop_n0inv, k->d_nth, k->ln, nwin, d_m, d_r, d_c, batch};
-  int grid; size_t smem;
-  coop_geometry(m->device, K, batch, &grid, &smem);
-  return rt_launch_coop(b, grid, 32 * COOP_WARPS, smem, s);
+  CoopEncBody<K> b{nullptr, 0, m->d_coop.p, m->coop_n0inv, k->d_nth, k->ln, nwin, d_m, d_r, d_c, batch};
+  return launch_coop<K>(b, batch, s);
 }
 template <int K>
 static int do_coop_decrypt_pow(pai_priv* k, const uint32_t* d_c, uint32_t* up, uint32_t* uq, long batch, rt_stream s) {
   const int L1 = 8 * k->NTP, L2 = 16 * k->NTP;
   CoopPowBody<K> b;
   b.consts = nullptr; b.const_quads = 0; b.nsides = 2;
-  b.blob[0] = k->p2->d_coop; b.blob[1] = k->q2->d_coop; b.n0inv[0] = k->p2->coop_n0inv; b.n0inv[1] = k->q2->coop_n0inv;
-  b.e[0] = k->d_coop_e; b.e[1] = k->d_coop_e + L1; b.e_limbs = L1;
+  b.blob[0] = k->p2->d_coop.p; b.blob[1] = k->q2->d_coop.p; b.n0inv[0] = k->p2->coop_n0inv; b.n0inv[1] = k->q2->coop_n0inv;
+  b.e[0] = k->d_coop_e.p; b.e[1] = k->d_coop_e.p + L1; b.e_limbs = L1;
   b.nwin[0] = (bit_length(h_sub_small(k->h_p, 1)) + COOP_W - 1) / COOP_W;
   b.nwin[1] = (bit_length(h_sub_small(k->h_q, 1)) + COOP_W - 1) / COOP_W;
   b.out[0] = up; b.out[1] = uq; b.base = d_c; b.base_limbs = 2 * L2; b.out_limbs = L2; b.batch = batch;
-  int grid; size_t smem;
-  coop_geometry(k->device, K, 2 * batch, &grid, &smem);
-  return rt_launch_coop(b, grid, 32 * COOP_WARPS, smem, s);
+  return launch_coop<K>(b, 2 * batch, s);
 }
 
 // ---- batched Miller-Rabin (key generation) -------------------------------------------------------
@@ -1293,39 +1232,96 @@ static int do_miller_rabin(const uint32_t* d_cand, const uint32_t* d_bases, int 
 #endif
   long blocks = (batch + nthr - 1) / nthr;
   int grid = (int)std::max(1L, std::min(blocks, (long)rt_sm_count(device) * 8));
-  void* ws = nullptr;
-  int rc = rt_malloc(&ws, (size_t)grid * nthr * mr_ws_limbs<NT, 4>() * 4);
+  TmpBuf ws;
+  int rc = ws.alloc((size_t)grid * nthr * mr_ws_limbs<NT, 4>() * 4);
   if (rc) return rc;
-  B body{nullptr, 0, d_cand, d_bases, rounds, d_result, (uint32_t*)ws, batch};
+  B body{nullptr, 0, d_cand, d_bases, rounds, d_result, ws.u32(), batch};
   rc = rt_launch(body, grid, nthr, 0, s);
   if (!rc) rc = rt_sync(s);
-  rt_free(ws);
   return rc;
 }
 
+// ---- one entry per operation and kernel family -------------------------------------------------------------------
 // rows per full wave of the throughput kernels (measured once per context from the launch geometry)
 static int pub_wave(pai_pub* k) {
+  if (k->wave) return 0;
   int rc = 0;
-  if (!k->wave) {
-    if (k->use_tc) { DISPATCH_TC(k->nmod->NT, k->wave = encrypt_wave_tc<NTH>(k)); }
-    else if (k->use_digit) { DISPATCH_NTH(k->nmod->NT, k->wave = encrypt_wave_digit<NTH>(k)); }
-    else { DISPATCH_NT(k->nsq->NT, k->wave = (wave_of<EncBody<NT>>(k->nsq->device, NT, mc_limbs(NT) / 4 + NT, 2))); }
-    if (rc) return rc;
-    if (k->wave <= 0) k->wave = 1;
+  switch (k->family) {
+    case TC: DISPATCH_TC(k->nmod->NT, k->wave = (tc_wave<TcEncBody<NTH>, NTH>(k->nmod->device, tc_enc_smem_bytes<NTH>))); break;
+    case DIGIT: DISPATCH_NTH(k->nmod->NT, k->wave = wave_of<EncDigitBody<NTH>>(k->nmod->device, enc_digit_shape<NTH>(k))); break;
+    case FULL: DISPATCH_NT(k->nsq->NT, k->wave = wave_of<EncBody<NT>>(k->nsq->device, enc_shape<NT>(k))); break;
   }
+  if (rc) return rc;
+  if (k->wave <= 0) k->wave = 1;
   return 0;
 }
 static int priv_wave(pai_priv* k) {
+  if (k->wave) return 0;
   int rc = 0;
-  if (!k->wave) {
-    if (k->use_tc) { DISPATCH_TC(k->NTP, k->wave = decrypt_wave_tc<NTH>(k)); }
-    else if (k->use_digit) { DISPATCH_NTP(k->NTP, k->wave = (wave_of<DecDigitBody<NTP, W_DEC>>(k->device, 2 * NTP, 2 * (dside_limbs<NTP>() / 4) + 2 * NTP, 2))); }
-    else { DISPATCH_NTP(k->NTP, k->wave = (wave_of<DecBody<NTP, W_DEC>>(k->device, 2 * NTP, 2 * (mc_limbs(2 * NTP) / 4 + mc_limbs(NTP) / 4 + 6 * NTP) + 2 * NTP, 3))); }
-    if (rc) return rc;
-    if (k->wave <= 0) k->wave = 1;
+  switch (k->family) {
+    case TC: DISPATCH_TC(k->NTP, k->wave = (tc_wave<TcDecBody<NTH, W_DEC>, NTH>(k->device, tc_dec_smem_bytes<NTH>))); break;
+    case DIGIT: DISPATCH_NTP(k->NTP, k->wave = (wave_of<DecDigitBody<NTP, W_DEC>>(k->device, dec_digit_shape<NTP>()))); break;
+    case FULL: DISPATCH_NTP(k->NTP, k->wave = (wave_of<DecBody<NTP, W_DEC>>(k->device, dec_shape<NTP>()))); break;
   }
+  if (rc) return rc;
+  if (k->wave <= 0) k->wave = 1;
   return 0;
 }
+// the throughput encrypt kernels on rows [0, batch) (after pub_wave)
+static int encrypt_rows(pai_pub* k, const uint32_t* d_m, const uint32_t* d_r, uint32_t* d_c, long batch, rt_stream s) {
+  int rc = 0;
+  switch (k->family) {
+    case TC:
+      DISPATCH_TC(k->nmod->NT, rc = tc_split(k->wave, batch, [&](long off, long rows) {
+        return do_encrypt_tc<NTH>(k, d_m + off * 8 * NTH, d_r + off * 8 * NTH, d_c + off * 16 * NTH, rows, s);
+      }));
+      break;
+    case DIGIT: DISPATCH_NTH(k->nmod->NT, rc = do_encrypt_digit<NTH>(k, d_m, d_r, d_c, batch, s)); break;
+    case FULL: DISPATCH_NT(k->nsq->NT, rc = do_encrypt<NT>(k, d_m, d_r, d_c, batch, s)); break;
+  }
+  return rc;
+}
+// the throughput decrypt kernels on rows [0, batch) (after priv_wave)
+static int decrypt_rows(pai_priv* k, const uint32_t* d_c, uint32_t* d_m, long batch, rt_stream s) {
+  int rc = 0;
+  switch (k->family) {
+    case TC:
+      DISPATCH_TC(k->NTP, rc = tc_split(k->wave, batch, [&](long off, long rows) {
+        return do_decrypt_tc<NTH>(k, d_c + off * 32 * NTH, d_m + off * 16 * NTH, rows, s);
+      }));
+      break;
+    case DIGIT: DISPATCH_NTP(k->NTP, rc = do_decrypt_digit<NTP>(k, d_c, d_m, batch, s)); break;
+    case FULL: DISPATCH_NTP(k->NTP, rc = do_decrypt<NTP>(k, d_c, d_m, batch, s)); break;
+  }
+  return rc;
+}
+
+namespace {
+struct StageIn { DevBuf<>& buf; const void* src; size_t bytes; };
+struct StageOut { DevBuf<>& buf; void* dst; size_t bytes; };   // dst may be null: the device result is not copied back
+// A host-pointer entry point: under the context's lock and on its device, copy the inputs into the context's staging
+// buffers, size the outputs, run `call` (the device-pointer variant on stream 0) and copy the outputs back.  The lock is
+// held until the results are in host memory.
+template <class Call>
+int run_staged(std::recursive_mutex& mu, int device, long batch, std::initializer_list<StageIn> in, std::initializer_list<StageOut> out,
+               Call call) {
+  DeviceGuard device_guard_; (void)device_guard_;
+  CtxLock lock_(mu);
+  if (batch == 0) return 0;
+  int rc = rt_set_device(device);
+  for (const StageIn& x : in) {
+    if (!rc) rc = x.buf.ensure(x.bytes);
+    if (!rc) rc = rt_h2d(x.buf.p, x.src, x.bytes, 0);
+  }
+  for (const StageOut& x : out) if (!rc) rc = x.buf.ensure(x.bytes);
+  if (!rc) rc = call();
+  for (const StageOut& x : out) if (!rc && x.dst) rc = rt_d2h(x.dst, x.buf.p, x.bytes, 0);
+  if (!rc) rc = rt_sync(0);
+  return rc;
+}
+template <class T = uint32_t>
+T* dev(const DevBuf<>& b) { return (T*)b.p; }
+}  // namespace
 
 extern "C" {
 
@@ -1338,7 +1334,7 @@ int pai_mod_create(const uint32_t* modulus, int limbs, int device, pai_mod** out
   DeviceGuard device_guard_; (void)device_guard_;
   return mod_create_impl(modulus, limbs, device, 0, 0, out);
 }
-int pai_mod_destroy(pai_mod* m) { mod_free(m); return 0; }
+int pai_mod_destroy(pai_mod* m) { mod_free(m, false); return 0; }
 int pai_mod_limbs(const pai_mod* m) { return m ? m->L : PAI_E_ARG; }
 
 int pai_mod_mulmod(pai_mod* m, const uint32_t* d_a, const uint32_t* d_b, uint32_t* d_out, long batch, void* stream) {
@@ -1348,7 +1344,7 @@ int pai_mod_mulmod(pai_mod* m, const uint32_t* d_a, const uint32_t* d_b, uint32_
   if (batch == 0) return 0;
   int rc = rt_set_device(m->device);
   if (rc) return rc;
-  DISPATCH_NT(m->NT, rc = do_mulmod<NT>(m, m->d_blob, mc_limbs(NT) / 4, d_a, d_b, d_out, batch, (rt_stream)stream));
+  DISPATCH_NT(m->NT, rc = do_mulmod<NT>(m, m->d_blob.p, mc_limbs(NT) / 4, d_a, d_b, d_out, batch, (rt_stream)stream));
   return rc;
 }
 
@@ -1429,7 +1425,7 @@ int pai_pub_create(const uint32_t* n, int limbs, int device, pai_pub** out) {
   int rc = mod_create_impl(nsq.data(), (int)nsq.size(), device, NT, ln, &k->nsq);
   if (rc) { delete k; return rc; }
   // n right after the blob (encrypt's constant area)
-  rc = rt_h2d(k->nsq->d_blob + mc_limbs(NT), nn.data(), (size_t)ln * 4, 0);
+  rc = rt_h2d(k->nsq->d_blob.p + mc_limbs(NT), nn.data(), (size_t)ln * 4, 0);
   // raw_mul branch threshold n - max_int, max_int = n//3 - 1   (phe/paillier.py:90, 745)
   limbs_t maxint = h_sub_small(h_div_small(nn, 3), 1);
   limbs_t thr = h_sub(nn, maxint);
@@ -1441,7 +1437,7 @@ int pai_pub_create(const uint32_t* n, int limbs, int device, pai_pub** out) {
   if (!rc) { DISPATCH_NTH(2 * ntp, rc = do_digit_setup<NTH>(k->nmod, 0)); }
   if (!rc) {   // compact encrypt constants: [ N | ONE | NINV | KL | RR | ZERO ] gathered from the digit blob
     const int h = 8 * 2 * ntp;
-    const uint32_t* b = k->nmod->d_blob;
+    const uint32_t* b = k->nmod->d_blob.p;
     const uint32_t* e = b + 5 * h + 8;            // KL | RR(2h) | ONEM(2h) | ZERO | ...
     rc = rt_malloc((void**)&k->d_enc_consts, (size_t)dc_pow_limbs(2 * ntp) * 4);
     uint32_t* c = k->d_enc_consts;
@@ -1452,14 +1448,12 @@ int pai_pub_create(const uint32_t* n, int limbs, int device, pai_pub** out) {
     if (!rc) rc = rt_d2d(c + 7 * h + 16, e + 3 * h, (size_t)2 * h * 4, 0);         // ONEM
     if (!rc) rc = rt_d2d(c + 9 * h + 16, e + 6 * h, (size_t)2 * h * 4, 0);         // E3
   }
-  { const char* e = getenv("PAI_ENCRYPT_PATH"); k->use_digit = !(e && std::string(e) == "full"); }
   // tensor-core reductions (pai_tc.cuh): digit moduli of at most 384 base-256 digits (keys up to 3072 bits; above that
   // the operand buffers of even one 128-thread group no longer fit shared memory)
-  if (!rc && tc_supported(2 * ntp, 12)) {
+  k->family = pick_family("PAI_ENCRYPT_PATH", tc_supported(2 * ntp, 12));
+  if (!rc && k->family == TC) {
     DISPATCH_TC(2 * ntp, rc = do_tc_setup<NTH>(k, 0));
-    k->use_tc = !rc && k->use_digit && tc_wanted();
-    const char* st = getenv("PAI_TC_STAGGER");
-    k->tc_stagger = st && *st ? atoi(st) : 40000;
+    k->tc_stagger = tc_stagger_cycles();
   }
   // exponent program for r^n: sliding windows of W_ENC bits over the public exponent n
   std::vector<uint32_t> prog = sliding_program(nn, W_ENC);
@@ -1480,14 +1474,14 @@ int pai_pub_destroy(pai_pub* k) {
   rt_free(k->d_enc_consts);
   rt_free(k->d_tc);
   k->ws.release(); k->h_m.release(); k->h_r.release(); k->h_c.release(); k->h_s.release();
-  mod_free(k->nsq);
-  mod_free(k->nmod);
+  mod_free(k->nsq, false);
+  mod_free(k->nmod, false);
   delete k;
   return 0;
 }
 int pai_pub_n_limbs(const pai_pub* k) { return k ? k->ln : PAI_E_ARG; }
 int pai_pub_c_limbs(const pai_pub* k) { return k ? 2 * k->ln : PAI_E_ARG; }
-int pai_pub_kernel_path(const pai_pub* k) { return !k ? PAI_E_ARG : (k->use_tc ? 2 : (k->use_digit ? 1 : 0)); }
+int pai_pub_kernel_path(const pai_pub* k) { return k ? k->family : PAI_E_ARG; }
 long pai_pub_wave(pai_pub* k) {
   DeviceGuard device_guard_; (void)device_guard_;
   if (!k) return PAI_E_ARG;
@@ -1516,10 +1510,7 @@ int pai_encrypt(pai_pub* k, const uint32_t* d_m, const uint32_t* d_r, uint32_t* 
     if (rc || off == 0) return rc;
     batch = off;
   }
-  if (k->use_tc) { DISPATCH_TC(k->nmod->NT, rc = do_encrypt_tc<NTH>(k, d_m, d_r, d_c, batch, (rt_stream)stream)); }
-  else if (k->use_digit) { DISPATCH_NTH(k->nmod->NT, rc = do_encrypt_digit<NTH>(k, d_m, d_r, d_c, batch, (rt_stream)stream)); }
-  else { DISPATCH_NT(k->nsq->NT, rc = do_encrypt<NT>(k, d_m, d_r, d_c, batch, (rt_stream)stream)); }
-  return rc;
+  return encrypt_rows(k, d_m, d_r, d_c, batch, (rt_stream)stream);
 }
 int pai_random_lt_n(pai_pub* k, const uint8_t* seed32, unsigned long long nonce, uint32_t* d_r, long batch, void* stream) {
   DeviceGuard device_guard_; (void)device_guard_;
@@ -1596,42 +1587,44 @@ int pai_raw_sum(pai_pub* k, const uint32_t* d_c, long batch, uint32_t* d_out, vo
   DISPATCH_NT(m->NT, rc = do_reduce_mul<NT>(m, d_c, batch, d_out, (rt_stream)stream));
   return rc;
 }
+// raw_mul's branch per element (phe/paillier.py:742-749) into the stream's workspace: exponent s or n - s (w_exp), base
+// c or invert(c) mod n^2 (w_base); statuses go to d_status, or to scratch when it is null
+static int rawmul_prepare(pai_pub* k, StreamWs& w, const uint32_t* d_a, const uint32_t* d_s, int32_t* d_status, long batch, rt_stream s) {
+  const int ln = k->ln;
+  int rc = w.w_exp.ensure((size_t)batch * ln * 4);
+  if (!rc) rc = w.w_base.ensure((size_t)batch * 2 * ln * 4);
+  if (!rc) rc = w.w_flag.ensure((size_t)batch * 4 * 2);
+  if (rc) return rc;
+  int32_t* flag = (int32_t*)w.w_flag.p;
+  PrepBody b{nullptr, 0, k->d_nth, k->d_nth + ln, ln, d_s, (uint32_t*)w.w_exp.p, flag, batch};
+  rc = rt_launch(b, (int)std::min((batch + 127) / 128, 65535L), 128, 0, s);
+  if (rc) return rc;
+  pai_mod* m = k->nsq;
+  DISPATCH_NT(m->NT, rc = do_invert_flagged<NT>(m, d_a, flag, (uint32_t*)w.w_base.p, d_status ? d_status : flag + batch, batch, s));
+  return rc;
+}
+// base^exp mod n^2 per element, exponents of ln limbs (raw_mul; raw_dot outside the tensor-core family)
+static int powers(pai_pub* k, const uint32_t* d_base, const uint32_t* d_exp, uint32_t* d_out, long batch, rt_stream s) {
+  int rc = 0;
+  switch (k->family) {
+    case TC: DISPATCH_TC(k->nmod->NT, rc = do_powmod_tc<NTH>(k, d_base, d_exp, k->ln, d_out, batch, s)); break;
+    case DIGIT: DISPATCH_NTH(k->nmod->NT, rc = do_powmod_digit<NTH>(k, d_base, d_exp, k->ln, d_out, batch, s)); break;
+    case FULL: rc = powmod_common(k->nsq, d_base, 2 * k->ln, d_exp, k->ln, k->ln, -1, d_out, batch, s); break;
+  }
+  return rc;
+}
 int pai_raw_mul(pai_pub* k, const uint32_t* d_a, const uint32_t* d_s, uint32_t* d_c, int32_t* d_status, long batch, void* stream) {
   DeviceGuard device_guard_; (void)device_guard_;
   if (!k || !d_a || !d_s || !d_c || batch < 0) { g_err = "bad argument"; return PAI_E_ARG; }
   CtxLock lock_(k->mu);
   if (batch == 0) return 0;
-  pai_mod* m = k->nsq;
   rt_stream s = (rt_stream)stream;
-  int rc = rt_set_device(m->device);
-  const int ln = k->ln, lc = 2 * k->ln;
+  int rc = rt_set_device(k->nsq->device);
+  if (rc) return rc;
   StreamWs& w = k->ws.get(s);
-  if (!rc) rc = w.w_exp.ensure((size_t)batch * ln * 4);
-  if (!rc) rc = w.w_base.ensure((size_t)batch * lc * 4);
-  if (!rc) rc = w.w_flag.ensure((size_t)batch * 4 * 2);
+  rc = rawmul_prepare(k, w, d_a, d_s, d_status, batch, s);
   if (rc) return rc;
-  int32_t* flag = (int32_t*)w.w_flag.p;
-  int32_t* status = d_status ? d_status : flag + batch;
-  // 1. branch test + exponent (s or n - s)
-  {
-    PrepBody b{nullptr, 0, k->d_nth, k->d_nth + ln, ln, d_s, (uint32_t*)w.w_exp.p, flag, batch};
-    long blocks = (batch + 127) / 128;
-    rc = rt_launch(b, (int)std::min(blocks, 65535L), 128, 0, s);
-    if (rc) return rc;
-  }
-  // 2. base = a, or invert(a, n^2) where flagged
-  DISPATCH_NT(m->NT, rc = do_invert_flagged<NT>(m, d_a, flag, (uint32_t*)w.w_base.p, status, batch, s));
-  if (rc) return rc;
-  // 3. base ^ exponent mod n^2
-  if (k->use_tc) {
-    DISPATCH_TC(k->nmod->NT, rc = do_powmod_tc<NTH>(k, (const uint32_t*)w.w_base.p, (const uint32_t*)w.w_exp.p, ln, d_c, batch, s));
-    return rc;
-  }
-  if (k->use_digit) {
-    DISPATCH_NTH(k->nmod->NT, rc = do_powmod_digit<NTH>(k, (const uint32_t*)w.w_base.p, (const uint32_t*)w.w_exp.p, ln, d_c, batch, s));
-    return rc;
-  }
-  return powmod_common(m, (const uint32_t*)w.w_base.p, lc, (const uint32_t*)w.w_exp.p, ln, ln, -1, d_c, batch, stream);
+  return powers(k, (const uint32_t*)w.w_base.p, (const uint32_t*)w.w_exp.p, d_c, batch, s);
 }
 
 int pai_raw_dot(pai_pub* k, const uint32_t* d_a, const uint32_t* d_s, uint32_t* d_out, int32_t* d_status, long batch, void* stream) {
@@ -1641,38 +1634,20 @@ int pai_raw_dot(pai_pub* k, const uint32_t* d_a, const uint32_t* d_s, uint32_t* 
   pai_mod* m = k->nsq;
   rt_stream s = (rt_stream)stream;
   int rc = rt_set_device(m->device);
-  const int ln = k->ln, lc = 2 * k->ln;
+  if (rc) return rc;
   StreamWs& w = k->ws.get(s);
-  if (!rc) rc = w.w_exp.ensure((size_t)batch * ln * 4);
-  if (!rc) rc = w.w_base.ensure((size_t)batch * lc * 4);
-  if (!rc) rc = w.w_flag.ensure((size_t)batch * 4 * 2);
+  rc = rawmul_prepare(k, w, d_a, d_s, d_status, batch, s);
+  if (!rc) rc = w.red_b.ensure((size_t)batch * 2 * k->ln * 4);   // a row per element (an upper bound for the Straus groups)
   if (rc) return rc;
-  int32_t* flag = (int32_t*)w.w_flag.p;
-  int32_t* status = d_status ? d_status : flag + batch;
-  {   // the reference's branch per element (phe/paillier.py:742-749): exponent s or n - s, base c or invert(c)
-    PrepBody b{nullptr, 0, k->d_nth, k->d_nth + ln, ln, d_s, (uint32_t*)w.w_exp.p, flag, batch};
-    long blocks = (batch + 127) / 128;
-    rc = rt_launch(b, (int)std::min(blocks, 65535L), 128, 0, s);
-    if (rc) return rc;
-  }
-  DISPATCH_NT(m->NT, rc = do_invert_flagged<NT>(m, d_a, flag, (uint32_t*)w.w_base.p, status, batch, s));
-  if (rc) return rc;
+  const uint32_t* base = (const uint32_t*)w.w_base.p;
+  const uint32_t* exp = (const uint32_t*)w.w_exp.p;
   long nrows = batch;
-  if (k->use_tc) {                                     // Straus groups on the tensor-core path -> one row per group
-    long ngroups = 0;
-    rc = w.red_b.ensure((size_t)batch * lc * 4);       // upper bound (gsz >= 1)
-    if (rc) return rc;
-    DISPATCH_TC(k->nmod->NT, rc = do_straus_tc<NTH>(k, (const uint32_t*)w.w_base.p, (const uint32_t*)w.w_exp.p, ln, batch,
-                                                    (uint32_t*)w.red_b.p, &ngroups, s));
-    if (rc) return rc;
-    nrows = ngroups;
-  } else {                                             // plain path: every power on its own, then the product
-    rc = w.red_b.ensure((size_t)batch * lc * 4);
-    if (rc) return rc;
-    if (k->use_digit) { DISPATCH_NTH(k->nmod->NT, rc = do_powmod_digit<NTH>(k, (const uint32_t*)w.w_base.p, (const uint32_t*)w.w_exp.p, ln, (uint32_t*)w.red_b.p, batch, s)); }
-    else rc = powmod_common(m, (const uint32_t*)w.w_base.p, lc, (const uint32_t*)w.w_exp.p, ln, ln, -1, (uint32_t*)w.red_b.p, batch, stream);
-    if (rc) return rc;
+  if (k->family == TC) {                               // Straus groups on the tensor-core path -> one row per group
+    DISPATCH_TC(k->nmod->NT, rc = do_straus_tc<NTH>(k, base, exp, k->ln, batch, (uint32_t*)w.red_b.p, &nrows, s));
+  } else {                                             // every power on its own, then the product
+    rc = powers(k, base, exp, (uint32_t*)w.red_b.p, batch, s);
   }
+  if (rc) return rc;
   CtxLock lock2_(m->mu);
   DISPATCH_NT(m->NT, rc = do_reduce_mul<NT>(m, (const uint32_t*)w.red_b.p, nrows, d_out, s));
   return rc;
@@ -1751,12 +1726,11 @@ int pai_priv_create(const uint32_t* p, const uint32_t* q, int limbs, int device,
   if (!rc) rc = mod_create_impl(qq.data(), L1, device, ntp, 0, &k->q1);
   if (!rc) { DISPATCH_NTP(ntp, rc = do_priv_setup<NTP>(k, 0)); }
   if (!rc) { DISPATCH_NTP(ntp, rc = do_priv_digit_setup<NTP>(k, 0)); }
-  { const char* e = getenv("PAI_DECRYPT_PATH"); k->use_digit = !(e && std::string(e) == "full"); }
-  if (!rc && tc_supported(ntp, 8)) {            // tensor-core reductions: p, q of 64 .. 256 base-256 digits (keys up to 4096 bits)
+  // tensor-core reductions: p, q of 64 .. 256 base-256 digits (keys up to 4096 bits)
+  k->family = pick_family("PAI_DECRYPT_PATH", tc_supported(ntp, 8));
+  if (!rc && k->family == TC) {
     DISPATCH_TC(ntp, rc = do_priv_tc_setup<NTH>(k, 0));
-    k->use_tc = !rc && k->use_digit && tc_wanted();
-    const char* st = getenv("PAI_TC_STAGGER");
-    k->tc_stagger = st && *st ? atoi(st) : 40000;
+    k->tc_stagger = tc_stagger_cycles();
   }
   if (rc) { pai_priv_destroy(k); return rc; }
   *out = k;
@@ -1765,30 +1739,16 @@ int pai_priv_create(const uint32_t* p, const uint32_t* q, int limbs, int device,
 int pai_priv_destroy(pai_priv* k) {
   if (!k) return 0;
   rt_set_device(k->device);
-  if (k->d_consts) {                      // wipe the secret constants before releasing them
-    const int sideq = mc_limbs(2 * k->NTP) / 4 + mc_limbs(k->NTP) / 4 + 6 * k->NTP;
-    rt_memset(k->d_consts, 0, ((size_t)2 * sideq + 2 * k->NTP) * 16, 0);
-    rt_sync(0);
-  }
-  rt_free(k->d_consts);
-  if (k->d_dconsts) {
-    const int L1 = 8 * k->NTP;
-    rt_memset(k->d_dconsts, 0, ((size_t)2 * (5 * L1 + 8 + 14 * L1 + 8 + 2 * L1) + L1) * 4, 0);
-    rt_sync(0);
-  }
-  rt_free(k->d_dconsts);
-  if (k->d_tc) { rt_memset(k->d_tc, 0, (size_t)2 * tc_blob_bytes(k->NTP), 0); rt_sync(0); rt_free(k->d_tc); }
-  if (k->d_coop_e) { rt_memset(k->d_coop_e, 0, (size_t)16 * k->NTP * 4, 0); rt_sync(0); rt_free(k->d_coop_e); }
-  mod_free(k->pd); mod_free(k->qd);
-  k->ws.release(); k->h_c.release(); k->h_m.release();
-  mod_free(k->p2); mod_free(k->q2); mod_free(k->p1); mod_free(k->q1);
-  std::fill(k->h_p.begin(), k->h_p.end(), 0); std::fill(k->h_q.begin(), k->h_q.end(), 0);
+  k->d_consts.release(true); k->d_dconsts.release(true); k->d_tc.release(true); k->d_coop_e.release(true);
+  k->ws.release(true); k->h_c.release(true); k->h_m.release(true);
+  for (pai_mod* m : {k->pd, k->qd, k->p2, k->q2, k->p1, k->q1}) mod_free(m, true);
+  for (limbs_t* h : {&k->h_p, &k->h_q, &k->h_pinv, &k->h_hp, &k->h_hq}) std::fill(h->begin(), h->end(), 0);
   delete k;
   return 0;
 }
 int pai_priv_n_limbs(const pai_priv* k) { return k ? 16 * k->NTP : PAI_E_ARG; }
 int pai_priv_c_limbs(const pai_priv* k) { return k ? 32 * k->NTP : PAI_E_ARG; }
-int pai_priv_kernel_path(const pai_priv* k) { return !k ? PAI_E_ARG : (k->use_tc ? 2 : (k->use_digit ? 1 : 0)); }
+int pai_priv_kernel_path(const pai_priv* k) { return k ? k->family : PAI_E_ARG; }
 long pai_priv_wave(pai_priv* k) {
   DeviceGuard device_guard_; (void)device_guard_;
   if (!k) return PAI_E_ARG;
@@ -1825,12 +1785,12 @@ int pai_decrypt(pai_priv* k, const uint32_t* d_c, uint32_t* d_m, long batch, voi
     const long off = batch - ncoop;
     rc = ensure_coop(k->p2, s);
     if (!rc) rc = ensure_coop(k->q2, s);
-    if (!rc && !k->d_coop_e) {
+    if (!rc && !k->d_coop_e.p) {
       limbs_t e = h_sub_small(k->h_p, 1), eq = h_sub_small(k->h_q, 1);
       e.resize(L1, 0); eq.resize(L1, 0);
       e.insert(e.end(), eq.begin(), eq.end());
-      rc = rt_malloc((void**)&k->d_coop_e, (size_t)2 * L1 * 4);
-      if (!rc) rc = rt_h2d(k->d_coop_e, e.data(), (size_t)2 * L1 * 4, s);
+      rc = k->d_coop_e.ensure((size_t)2 * L1 * 4);
+      if (!rc) rc = rt_h2d(k->d_coop_e.p, e.data(), (size_t)2 * L1 * 4, s);
       if (!rc) rc = rt_sync(s);
     }
     StreamWs& w = k->ws.get(s);
@@ -1844,132 +1804,57 @@ int pai_decrypt(pai_priv* k, const uint32_t* d_c, uint32_t* d_m, long batch, voi
     if (rc || off == 0) return rc;
     batch = off;
   }
-  if (k->use_tc) { DISPATCH_TC(k->NTP, rc = do_decrypt_tc<NTH>(k, d_c, d_m, batch, (rt_stream)stream)); }
-  else if (k->use_digit) { DISPATCH_NTP(k->NTP, rc = do_decrypt_digit<NTP>(k, d_c, d_m, batch, (rt_stream)stream)); }
-  else { DISPATCH_NTP(k->NTP, rc = do_decrypt<NTP>(k, d_c, d_m, batch, (rt_stream)stream)); }
-  return rc;
+  return decrypt_rows(k, d_c, d_m, batch, (rt_stream)stream);
 }
 
 // ---------------------------------------------------------------------------------------- host-pointer variants
-#define STAGE_IN(buf, host, bytes) do { rc = (buf).ensure(bytes); if (!rc) rc = rt_h2d((buf).p, host, bytes, 0); if (rc) return rc; } while (0)
 
 int pai_encrypt_host(pai_pub* k, const uint32_t* m, const uint32_t* r, uint32_t* c, long batch) {
-  DeviceGuard device_guard_; (void)device_guard_;
   if (!k || !m || !r || !c || batch < 0) { g_err = "bad argument"; return PAI_E_ARG; }
-  CtxLock lock_(k->mu);
-  if (batch == 0) return 0;
-  int rc = rt_set_device(k->nsq->device);
-  if (rc) return rc;
-  size_t bn = (size_t)batch * k->ln * 4;
-  STAGE_IN(k->h_m, m, bn);
-  STAGE_IN(k->h_r, r, bn);
-  rc = k->h_c.ensure(2 * bn);
-  if (!rc) rc = pai_encrypt(k, (const uint32_t*)k->h_m.p, (const uint32_t*)k->h_r.p, (uint32_t*)k->h_c.p, batch, nullptr);
-  if (!rc) rc = rt_d2h(c, k->h_c.p, 2 * bn, 0);
-  if (!rc) rc = rt_sync(0);
-  return rc;
+  const size_t bn = (size_t)batch * k->ln * 4;
+  return run_staged(k->mu, k->nsq->device, batch, {{k->h_m, m, bn}, {k->h_r, r, bn}}, {{k->h_c, c, 2 * bn}},
+                    [&] { return pai_encrypt(k, dev(k->h_m), dev(k->h_r), dev(k->h_c), batch, nullptr); });
 }
 int pai_raw_add_host(pai_pub* k, const uint32_t* a, const uint32_t* b, uint32_t* c, long batch) {
-  DeviceGuard device_guard_; (void)device_guard_;
   if (!k || !a || !b || !c || batch < 0) { g_err = "bad argument"; return PAI_E_ARG; }
-  CtxLock lock_(k->mu);
-  if (batch == 0) return 0;
-  int rc = rt_set_device(k->nsq->device);
-  if (rc) return rc;
-  size_t bc = (size_t)batch * 2 * k->ln * 4;
-  STAGE_IN(k->h_m, a, bc);
-  STAGE_IN(k->h_r, b, bc);
-  rc = k->h_c.ensure(bc);
-  if (!rc) rc = pai_raw_add(k, (const uint32_t*)k->h_m.p, (const uint32_t*)k->h_r.p, (uint32_t*)k->h_c.p, batch, nullptr);
-  if (!rc) rc = rt_d2h(c, k->h_c.p, bc, 0);
-  if (!rc) rc = rt_sync(0);
-  return rc;
+  const size_t bc = (size_t)batch * 2 * k->ln * 4;
+  return run_staged(k->mu, k->nsq->device, batch, {{k->h_m, a, bc}, {k->h_r, b, bc}}, {{k->h_c, c, bc}},
+                    [&] { return pai_raw_add(k, dev(k->h_m), dev(k->h_r), dev(k->h_c), batch, nullptr); });
 }
 int pai_raw_mul_host(pai_pub* k, const uint32_t* a, const uint32_t* s, uint32_t* c, int32_t* status, long batch) {
-  DeviceGuard device_guard_; (void)device_guard_;
   if (!k || !a || !s || !c || batch < 0) { g_err = "bad argument"; return PAI_E_ARG; }
-  CtxLock lock_(k->mu);
-  if (batch == 0) return 0;
-  int rc = rt_set_device(k->nsq->device);
-  if (rc) return rc;
-  size_t bn = (size_t)batch * k->ln * 4;
-  STAGE_IN(k->h_m, a, 2 * bn);
-  STAGE_IN(k->h_s, s, bn);
-  rc = k->h_c.ensure(2 * bn);
-  if (!rc) rc = k->h_r.ensure((size_t)batch * 4);
-  if (!rc) rc = pai_raw_mul(k, (const uint32_t*)k->h_m.p, (const uint32_t*)k->h_s.p, (uint32_t*)k->h_c.p, (int32_t*)k->h_r.p, batch, nullptr);
-  if (!rc) rc = rt_d2h(c, k->h_c.p, 2 * bn, 0);
-  if (!rc && status) rc = rt_d2h(status, k->h_r.p, (size_t)batch * 4, 0);
-  if (!rc) rc = rt_sync(0);
-  return rc;
+  const size_t bn = (size_t)batch * k->ln * 4;
+  return run_staged(k->mu, k->nsq->device, batch, {{k->h_m, a, 2 * bn}, {k->h_s, s, bn}}, {{k->h_c, c, 2 * bn}, {k->h_r, status, (size_t)batch * 4}},
+                    [&] { return pai_raw_mul(k, dev(k->h_m), dev(k->h_s), dev(k->h_c), dev<int32_t>(k->h_r), batch, nullptr); });
 }
 int pai_decrypt_host(pai_priv* k, const uint32_t* c, uint32_t* m, long batch) {
-  DeviceGuard device_guard_; (void)device_guard_;
   if (!k || !c || !m || batch < 0) { g_err = "bad argument"; return PAI_E_ARG; }
-  CtxLock lock_(k->mu);
-  if (batch == 0) return 0;
-  int rc = rt_set_device(k->device);
-  if (rc) return rc;
-  size_t bn = (size_t)batch * 16 * k->NTP * 4;
-  STAGE_IN(k->h_c, c, 2 * bn);
-  rc = k->h_m.ensure(bn);
-  if (!rc) rc = pai_decrypt(k, (const uint32_t*)k->h_c.p, (uint32_t*)k->h_m.p, batch, nullptr);
-  if (!rc) rc = rt_d2h(m, k->h_m.p, bn, 0);
-  if (!rc) rc = rt_sync(0);
-  return rc;
+  const size_t bn = (size_t)batch * 16 * k->NTP * 4;
+  return run_staged(k->mu, k->device, batch, {{k->h_c, c, 2 * bn}}, {{k->h_m, m, bn}},
+                    [&] { return pai_decrypt(k, dev(k->h_c), dev(k->h_m), batch, nullptr); });
 }
 int pai_mod_mulmod_host(pai_mod* m, const uint32_t* a, const uint32_t* b, uint32_t* out, long batch) {
-  DeviceGuard device_guard_; (void)device_guard_;
   if (!m || !a || !b || !out || batch < 0) { g_err = "bad argument"; return PAI_E_ARG; }
-  CtxLock lock_(m->mu);
-  if (batch == 0) return 0;
-  int rc = rt_set_device(m->device);
-  if (rc) return rc;
-  size_t bl = (size_t)batch * m->L * 4;
-  STAGE_IN(m->tmp_a, a, bl);
-  STAGE_IN(m->tmp_b, b, bl);
-  rc = m->tmp_o.ensure(bl);
-  if (!rc) rc = pai_mod_mulmod(m, (const uint32_t*)m->tmp_a.p, (const uint32_t*)m->tmp_b.p, (uint32_t*)m->tmp_o.p, batch, nullptr);
-  if (!rc) rc = rt_d2h(out, m->tmp_o.p, bl, 0);
-  if (!rc) rc = rt_sync(0);
-  return rc;
+  const size_t bl = (size_t)batch * m->L * 4;
+  return run_staged(m->mu, m->device, batch, {{m->tmp_a, a, bl}, {m->tmp_b, b, bl}}, {{m->tmp_o, out, bl}},
+                    [&] { return pai_mod_mulmod(m, dev(m->tmp_a), dev(m->tmp_b), dev(m->tmp_o), batch, nullptr); });
 }
 int pai_mod_powmod_host(pai_mod* m, const uint32_t* base, int base_limbs, const uint32_t* exp, int exp_limbs, int shared_exp,
                         uint32_t* out, long batch) {
-  DeviceGuard device_guard_; (void)device_guard_;
   if (!m || !base || !exp || !out || batch < 0) { g_err = "bad argument"; return PAI_E_ARG; }
-  CtxLock lock_(m->mu);
-  if (batch == 0) return 0;
-  int rc = rt_set_device(m->device);
-  if (rc) return rc;
-  STAGE_IN(m->tmp_a, base, (size_t)batch * base_limbs * 4);
-  rc = m->tmp_o.ensure((size_t)batch * m->L * 4);
-  if (rc) return rc;
-  if (shared_exp) {
-    rc = pai_mod_powmod_shared(m, (const uint32_t*)m->tmp_a.p, base_limbs, exp, exp_limbs, (uint32_t*)m->tmp_o.p, batch, nullptr);
-  } else {
-    STAGE_IN(m->tmp_b, exp, (size_t)batch * exp_limbs * 4);
-    rc = pai_mod_powmod(m, (const uint32_t*)m->tmp_a.p, base_limbs, (const uint32_t*)m->tmp_b.p, exp_limbs, (uint32_t*)m->tmp_o.p, batch, nullptr);
-  }
-  if (!rc) rc = rt_d2h(out, m->tmp_o.p, (size_t)batch * m->L * 4, 0);
-  if (!rc) rc = rt_sync(0);
-  return rc;
+  const size_t bb = (size_t)batch * base_limbs * 4, bo = (size_t)batch * m->L * 4;
+  if (shared_exp)     // the exponent stays in host memory (pai_mod_powmod_shared)
+    return run_staged(m->mu, m->device, batch, {{m->tmp_a, base, bb}}, {{m->tmp_o, out, bo}}, [&] {
+      return pai_mod_powmod_shared(m, dev(m->tmp_a), base_limbs, exp, exp_limbs, dev(m->tmp_o), batch, nullptr);
+    });
+  return run_staged(m->mu, m->device, batch, {{m->tmp_a, base, bb}, {m->tmp_b, exp, (size_t)batch * exp_limbs * 4}}, {{m->tmp_o, out, bo}},
+                    [&] { return pai_mod_powmod(m, dev(m->tmp_a), base_limbs, dev(m->tmp_b), exp_limbs, dev(m->tmp_o), batch, nullptr); });
 }
 int pai_mod_invert_host(pai_mod* m, const uint32_t* a, int a_limbs, uint32_t* out, int32_t* status, long batch) {
-  DeviceGuard device_guard_; (void)device_guard_;
   if (!m || !a || !out || batch < 0) { g_err = "bad argument"; return PAI_E_ARG; }
-  CtxLock lock_(m->mu);
-  if (batch == 0) return 0;
-  int rc = rt_set_device(m->device);
-  if (rc) return rc;
-  STAGE_IN(m->tmp_a, a, (size_t)batch * a_limbs * 4);
-  rc = m->tmp_o.ensure((size_t)batch * m->L * 4);
-  if (!rc) rc = m->tmp_s.ensure((size_t)batch * 4);
-  if (!rc) rc = pai_mod_invert(m, (const uint32_t*)m->tmp_a.p, a_limbs, (uint32_t*)m->tmp_o.p, (int32_t*)m->tmp_s.p, batch, nullptr);
-  if (!rc) rc = rt_d2h(out, m->tmp_o.p, (size_t)batch * m->L * 4, 0);
-  if (!rc && status) rc = rt_d2h(status, m->tmp_s.p, (size_t)batch * 4, 0);
-  if (!rc) rc = rt_sync(0);
-  return rc;
+  return run_staged(m->mu, m->device, batch, {{m->tmp_a, a, (size_t)batch * a_limbs * 4}},
+                    {{m->tmp_o, out, (size_t)batch * m->L * 4}, {m->tmp_s, status, (size_t)batch * 4}},
+                    [&] { return pai_mod_invert(m, dev(m->tmp_a), a_limbs, dev(m->tmp_o), dev<int32_t>(m->tmp_s), batch, nullptr); });
 }
 
 }  // extern "C"
