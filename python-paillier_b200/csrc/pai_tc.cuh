@@ -4,11 +4,11 @@
 //     m = T_lo * N' mod R        (N' = -n^-1 mod R)          and          hi = floor(m * n / R).
 // In base-256 digits, for the 128 ciphertexts of a thread group (one warpgroup) at once, that is  [128 x D] x Toeplitz(const):
 // wgmma.mma_async u8 x u8 -> s32 GEMMs (two m64 halves of the 128 rows, K = 32 digits per instruction, column sums
-// <= D * 255^2 < 2^24).  The accumulator fragments are computed 32 columns at a time and moved by warp shuffles to the
-// lane that owns the row, which propagates the carries (ALU pipe) and has the quotient / the high half as ordinary 32-bit
-// limbs again.  What stays on the integer-multiply pipe are only the products of two per-ciphertext numbers (x0*y0,
-// x0*y1 + x1*y0): 100 instead of 228 tile products per squaring, 192 instead of 320 per multiplication at 2048-bit keys,
-// and no quotient products.
+// <= D * 255^2 < 2^25; at D = 384 they pass 2^24, and tc_limbs8 keeps the high word of every shifted sum).  The
+// accumulator fragments are computed 32 columns at a time and moved by warp shuffles to the lane that owns the row, which
+// propagates the carries (ALU pipe) and has the quotient / the high half as ordinary 32-bit limbs again.  What stays on
+// the integer-multiply pipe are only the products of two per-ciphertext numbers (x0*y0, x0*y1 + x1*y0): 100 instead of
+// 228 tile products per squaring, 192 instead of 320 per multiplication at 2048-bit keys, and no quotient products.
 //
 // Exactness of the high half.  GEMM 2 produces the byte columns D-4 .. 2D-5 of m*n (the top three columns 2D-4 .. 2D-2
 // are six scalar byte products).  The columns below D-4 are never computed: their sum I is < 1.004 * 256^(D-2), and the
@@ -255,7 +255,7 @@ PAI_DEV void tc_gemm(TcCtx<NTH>& c, int which) {
   TC_EACH_ROW {
     const int r = c.row0 + rw;
     for (int j = 0; j < D; j++) {
-      uint32_t sum = 0;                                   // <= D * 255^2 < 2^24
+      uint32_t sum = 0;                                   // <= D * 255^2 < 2^25
       for (int kap = 0; kap < NTH; kap++) {
         const int u0 = D - 32 - 32 * kap;
         for (int h = 0; h < 2; h++) {                     // 16 contiguous digits of the row x 16 contiguous band bytes
@@ -278,9 +278,11 @@ PAI_DEV void tc_gemm(TcCtx<NTH>& c, int which) {
 #endif
 }
 
-// eight 32-bit limbs from 32 byte-column sums (each < 2^24) and the running carry.
+// eight 32-bit limbs from 32 byte-column sums (any 32-bit values) and the running carry.
 // On the GPU this is spelled in funnel shifts and add-with-carry chains so that it runs on the ALU pipe: written as 64-bit
 // C arithmetic ptxas turned the shifts into IMAD.WIDE (three per limb), i.e. onto the very pipe the products need.
+// The high word of every shifted sum is kept: at D = 384 digits (3072-bit n) a column sum reaches 384 * 255^2 > 2^24, so
+// v1 << 8 has a high part too.
 PAI_DEV void tc_limbs8(const uint32_t v[32], uint32_t& carry, uint32_t out[8]) {
   PAI_UNROLL
   for (int j = 0; j < 8; j++) {
@@ -290,8 +292,9 @@ PAI_DEV void tc_limbs8(const uint32_t v[32], uint32_t& carry, uint32_t out[8]) {
     carry = (uint32_t)(x >> 32);
 #else
     uint32_t lo, hi;
-    asm("{\n\t.reg .u32 t1, t2, t3, h2, h3;\n\t"
-        "shf.l.wrap.b32 t1, 0, %3, 8;\n\t"          // v1 << 8   (v1 < 2^24: no high part)
+    asm("{\n\t.reg .u32 t1, t2, t3, h1, h2, h3;\n\t"
+        "shf.l.wrap.b32 t1, 0, %3, 8;\n\t"          // low word of v1 << 8
+        "shf.r.wrap.b32 h1, %3, 0, 24;\n\t"         // v1 >> 24
         "shf.l.wrap.b32 t2, 0, %4, 16;\n\t"         // low word of v2 << 16
         "shf.r.wrap.b32 h2, %4, 0, 16;\n\t"         // v2 >> 16
         "shf.l.wrap.b32 t3, 0, %5, 24;\n\t"         // low word of v3 << 24
@@ -299,7 +302,7 @@ PAI_DEV void tc_limbs8(const uint32_t v[32], uint32_t& carry, uint32_t out[8]) {
         "add.cc.u32 %0, %2, t1;\n\t"
         "addc.u32 %1, h2, h3;\n\t"
         "add.cc.u32 %0, %0, t2;\n\t"
-        "addc.u32 %1, %1, 0;\n\t"
+        "addc.u32 %1, %1, h1;\n\t"
         "add.cc.u32 %0, %0, t3;\n\t"
         "addc.u32 %1, %1, 0;\n\t"
         "add.cc.u32 %0, %0, %6;\n\t"
