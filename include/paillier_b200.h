@@ -154,6 +154,16 @@ int pai_priv_kernel_path(const pai_priv* k);   /* as pai_pub_kernel_path (tensor
 int pai_priv_get(const pai_priv* k, uint32_t* p, uint32_t* q, uint32_t* p_inverse, uint32_t* hp, uint32_t* hq);
 /* m[i] = raw_decrypt(c[i]) with CRT             phe/paillier.py:328-374 */
 int pai_decrypt(pai_priv* k, const uint32_t* d_c, uint32_t* d_m, long batch, void* stream);
+/* c[i] = (1 + n*m[i]) * r[i]^n mod n^2 for whatever integers the rows hold: the value pai_encrypt returns for the same
+ * integers, bit for bit, computed with the private key.  m, r: [batch][pai_priv_n_limbs()]; c: [batch][pai_priv_c_limbs()]
+ * (the layout of pai_decrypt).  The key holder's encryption: r^n mod p^2 and mod q^2 from half-length exponentiations
+ * (s = (r mod x)^(y mod (x-1)) mod x, then s^x mod x^2 for x, y = p, q and q, p), the message factor per prime, and
+ * Garner's CRT to n^2.  Secret exponents run through fixed windows with no digit skipped.  The result is defined for
+ * prime p and q, like pai_decrypt's; pai_priv_create does not test primality.  The per-key constants are derived on the
+ * first call.  Small batches and the tail beyond whole waves take warp-per-ciphertext exponentiations (PAI_COOP_MAX as
+ * for pai_encrypt).  Always on the integer-pipe digit kernels, whatever PAI_TC / PAI_DECRYPT_PATH select.  Asynchronous
+ * on `stream`, except for the first call, which waits for the constants' upload. */
+int pai_priv_encrypt(pai_priv* k, const uint32_t* d_m, const uint32_t* d_r, uint32_t* d_c, long batch, void* stream);
 
 /* ---- decimal wire format: the radix conversion behind the reference's JSON serialisation ---------
  * (docs/serialisation.rst:24-42 ships ciphertexts as str(int); phe/command_line.py:120-131, 267-276 likewise.)
@@ -180,6 +190,7 @@ int pai_encrypt_host(pai_pub* k, const uint32_t* m, const uint32_t* r, uint32_t*
 int pai_raw_add_host(pai_pub* k, const uint32_t* a, const uint32_t* b, uint32_t* c, long batch);
 int pai_raw_mul_host(pai_pub* k, const uint32_t* a, const uint32_t* s, uint32_t* c, int32_t* status, long batch);
 int pai_decrypt_host(pai_priv* k, const uint32_t* c, uint32_t* m, long batch);
+int pai_priv_encrypt_host(pai_priv* k, const uint32_t* m, const uint32_t* r, uint32_t* c, long batch);
 int pai_mod_mulmod_host(pai_mod* m, const uint32_t* a, const uint32_t* b, uint32_t* out, long batch);
 int pai_mod_powmod_host(pai_mod* m, const uint32_t* base, int base_limbs, const uint32_t* exp, int exp_limbs, int shared_exp,
                         uint32_t* out, long batch);

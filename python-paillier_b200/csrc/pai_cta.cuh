@@ -664,6 +664,29 @@ PAI_DEV void cta_decrypt_digit(u4* smem, const CtaId& id, int nwin_p, int nwin_q
   }
 }
 
+// ---- encrypt with the private key in digit form (pai_priv_encrypt).  consts = pe_const_limbs<NTP>(); two buffers of
+// 2*NTP tiles per thread and the static chunks of cta_decrypt_digit.  pre_p / pre_q: r^n mod p^2 / q^2 from the warp
+// kernels (then no ladder runs), or null.
+template <int NTP, int W>
+PAI_DEV void cta_priv_encrypt_digit(u4* smem, const CtaId& id, int nwin_p, int nwin_q, const uint32_t* m, const uint32_t* r,
+                                    const uint32_t* pre_p, const uint32_t* pre_q, uint32_t* out, long batch, u4* tbl) {
+  PEncC<NTP> C;
+  pe_bind<NTP>(C, smem, nwin_p, nwin_q);
+  DPowEnv<NTP> E;
+  cta_bufs<2 * NTP>(E.buf, 2, smem, pe_const_limbs<NTP>() / 4, id);
+  E.tbl = cta_table_slots<2 * NTP>(tbl, id, pe_slots(W));
+  E.dc = &C.P.dc;
+  E.step_sync = 1;
+  const int ln = 16 * NTP, lc = 32 * NTP;
+  for (long chunk = id.cta; chunk * id.nthr < batch; chunk += id.ncta) {
+    long g = chunk * id.nthr + id.tid;
+    bool store = g < batch;
+    if (!store) g = batch - 1;
+    prog_priv_encrypt_digit<NTP, W>(E, C, m + g * ln, r + g * ln, pre_p ? pre_p + g * ln : nullptr, pre_q ? pre_q + g * ln : nullptr,
+                                    out + g * lc, store);
+  }
+}
+
 
 // ---- c^k mod n^2 in digit form (raw_mul).  consts = compact constants with ONEM and E3 (dc_pow_limbs).
 // Exponents differ per element; the window count is made CTA-uniform (max over the CTA through one shared word)

@@ -723,6 +723,196 @@ PAI_DEV void prog_decrypt_digit(DPowEnv<NTP>& E, DSideC<NTP>& P, DSideC<NTP>& Qs
 
 
 // ------------------------------------------------------------------------------------------------
+// Encryption with the private key (pai_priv_encrypt): c = (1 + n*m) * r^n mod n^2 through the CRT, n = p*q with p < q.
+// For x in {p, q} and y the other prime:
+//   r^n = (r^x)^y = s^x (mod x^2),  s = (r mod x)^(y mod (x-1)) mod x     (x-th powers mod x^2 depend on r mod x only,
+//                                                                          and r^x mod x^2 has order dividing x - 1)
+//   1 + n*m = 1 + x*((y*m) mod x)  (mod x^2): the plain digit pair (1, t_x), t_x = y*m mod x
+//   c = c_p + p^2 * h,  h = (c_q - c_p) * p^-2 mod q^2                    (Garner; c_p < p^2 < q^2, so c < n^2 as it stands)
+// Both exponents are secret and run through fixed windows with no digit skipped.  x | r gives s = 0 (y mod (x-1) >= 1),
+// hence r^n = 0 mod x^2, as it must.
+// The warp-per-ciphertext route computes r^n mod x^2 as r^(n mod x(x-1)) on the warp kernels and passes the plain results
+// in (pre_p / pre_q): n mod x(x-1) = x * (y mod (x-1)) >= x, so that form holds for every r, x | r included.
+// Constants of one side:  [ digit blob of x (dc_limbs) | yR = y*R mod x | yR2 = y*R^2 mod x | e1 = y mod (x-1) ]
+// after the two sides:    [ K1 = p^-2*R | K1N = -p^-2*R | K2N = -p^-2*R^2 (mod q^2, digit pairs [d0 | d1]) | P2 = p^2 (plain) ]
+template <int NTH>
+PAI_DEV void digit_enter(const DPowEnv<NTH>& E, const uint32_t* base_row);
+
+template <int NTP>
+struct PESideC {
+  DigitEnv dc;
+  Opnd R1, R2, R3;    // R^k mod x (blob of x)
+  Opnd yR, yR2;
+  const uint32_t* e1;
+  int nwin;           // windows of both exponents (bit length of x)
+};
+template <int NTP>
+struct PEncC {
+  PESideC<NTP> P, Q;
+  DNum K1, K1N, K2N;
+  Opnd P2;
+};
+template <int NTP>
+PAI_HD int pe_side_limbs() { return dc_limbs(NTP) + 3 * 8 * NTP; }
+template <int NTP>
+PAI_HD int pe_const_limbs() { return 2 * pe_side_limbs<NTP>() + 4 * 16 * NTP; }
+// table slots per thread: the 2^W window entries, then [t_p | t_q] and the parked c_p
+PAI_HD int pe_slots(int W) { return (1 << W) + 2; }
+
+template <int NTP>
+PAI_DEV void pe_side_bind(PESideC<NTP>& S, u4* base, int nwin) {
+  const int Q = 2 * NTP;
+  digit_bind<NTP>(S.dc, base);
+  S.R1.p = base + Q;          S.R1.s = 1;
+  S.R2.p = base + 2 * Q;      S.R2.s = 1;
+  S.R3.p = base + 3 * Q;      S.R3.s = 1;
+  u4* p = base + dc_limbs(NTP) / 4;
+  S.yR.p = p;                 S.yR.s = 1;
+  S.yR2.p = p + Q;            S.yR2.s = 1;
+  S.e1 = (const uint32_t*)(p + 2 * Q);
+  S.nwin = nwin;
+}
+template <int NTP>
+PAI_DEV void pe_bind(PEncC<NTP>& C, u4* smem, int nwin_p, int nwin_q) {
+  const int Q = 2 * NTP;
+  pe_side_bind<NTP>(C.P, smem, nwin_p);
+  pe_side_bind<NTP>(C.Q, smem + pe_side_limbs<NTP>() / 4, nwin_q);
+  u4* k = smem + 2 * (pe_side_limbs<NTP>() / 4);
+  DNum* ks[3] = {&C.K1, &C.K1N, &C.K2N};
+  for (int i = 0; i < 3; i++) {
+    ks[i]->d0.p = k + 2 * i * Q;       ks[i]->d0.s = 1;
+    ks[i]->d1.p = k + (2 * i + 1) * Q; ks[i]->d1.s = 1;
+  }
+  C.P2.p = k + 6 * Q;         C.P2.s = 1;
+}
+
+// t = y*m mod x = m0*yR/R + m1*yR2/R (m = m0 + m1*R, any m < R^2); tmp: NTP tiles of scratch
+template <int NTP>
+PAI_DEV void pe_msg_digit(const Opnd& t, const Opnd& tmp, const PESideC<NTP>& S, const uint32_t* m_row) {
+  Opnd m0{(u4*)m_row, 1}, m1{(u4*)(m_row + 8 * NTP), 1};
+  mont_mul<NTP>(t, m0, S.yR, S.dc.N, S.dc.NI);
+  mont_mul<NTP>(tmp, m1, S.yR2, S.dc.N, S.dc.NI);
+  uint32_t c = big_add_masked<NTP>(t, t, tmp, 0xffffffffu);
+  big_cond_sub<NTP>(t, S.dc.N, c);
+}
+
+// Step 1: base^e * R mod x by fixed windows (no digit skipped) on half-width operands.  The base (Montgomery form mod x)
+// is in the low half of buf[0]; window entry i is the low half of table slot i.  Returns the operand holding the result.
+template <int NTP, int W>
+PAI_DEV Opnd mpow_fixed(const DPowEnv<NTP>& E, const PESideC<NTP>& S, const uint32_t* e, int nwin) {
+  const Opnd N = S.dc.N, NI = S.dc.NI;
+  const Opnd b = half_lo<NTP>(E.buf[0]);
+  Opnd cur = half_lo<NTP>(E.buf[1]), oth = half_hi<NTP>(E.buf[1]);
+  big_copy<NTP>(dtbl_entry<NTP>(E, 0).d0, S.R1);
+  big_copy<NTP>(dtbl_entry<NTP>(E, 1).d0, b);
+  mont_sqr<NTP>(cur, b, N, NI);
+  big_copy<NTP>(dtbl_entry<NTP>(E, 2).d0, cur);
+  for (int i = 3; i < (1 << W); i++) {
+    mont_mul<NTP>(oth, cur, b, N, NI);
+    { Opnd t = cur; cur = oth; oth = t; }
+    big_copy<NTP>(dtbl_entry<NTP>(E, i).d0, cur);
+  }
+  big_copy<NTP>(cur, dtbl_entry<NTP>(E, (int)exp_digit(e, 8 * NTP, (nwin - 1) * W, W)).d0);
+  for (int wi = nwin - 2; wi >= 0; wi--) {
+    for (int s = 0; s < W; s++) {
+      if (E.step_sync) cta_step_sync();
+      mont_sqr<NTP>(oth, cur, N, NI);
+      Opnd t = cur; cur = oth; oth = t;
+    }
+    if (E.step_sync) cta_step_sync();
+    mont_mul<NTP>(oth, cur, dtbl_entry<NTP>(E, (int)exp_digit(e, 8 * NTP, wi * W, W)).d0, N, NI);
+    Opnd t = cur; cur = oth; oth = t;
+  }
+  return cur;
+}
+
+// r^n mod x^2 in Montgomery digit form -> (buf[ret], orientation *sw).  r = r0 + r1*R (any r < R^2).
+template <int NTP, int W>
+PAI_DEV int pe_pow_side(DPowEnv<NTP>& E, PESideC<NTP>& S, const uint32_t* r_row, int* sw) {
+  DigitEnv& dc = S.dc;
+  E.dc = &dc;
+  Opnd r0{(u4*)r_row, 1}, r1{(u4*)(r_row + 8 * NTP), 1};
+  const Opnd a = half_lo<NTP>(E.buf[0]), t = half_hi<NTP>(E.buf[0]), u = half_lo<NTP>(E.buf[1]);
+  mont_mul<NTP>(t, r0, S.R2, dc.N, dc.NI);                                // r0 * R
+  mont_mul<NTP>(u, r1, S.R3, dc.N, dc.NI);                                // r1 * R^2
+  uint32_t c = big_add_masked<NTP>(a, t, u, 0xffffffffu);
+  big_cond_sub<NTP>(a, dc.N, c);                                          // r * R mod x
+  const Opnd s = mpow_fixed<NTP, W>(E, S, S.e1, S.nwin);                  // s * R mod x
+  // (s*R mod x, 0) read as a Montgomery digit pair stands for some s' = s (mod x), and s'^x = s^x (mod x^2)
+  big_copy<NTP>(a, s);
+  big_copy<NTP>(t, dc.ZERO);
+  return dpow_fixed<NTP, W>(E, 0, 0, (const uint32_t*)dc.N.p, 8 * NTP, S.nwin, sw);   // s^x * R mod x^2
+}
+
+// The tail shared by the thread-per-ciphertext and the warp-per-ciphertext routes.  Side p: c_p = omega_p * (1, t_p) as a
+// plain number, parked in table slot 2^W + 1.  omega: r^n mod p^2 in Montgomery digit form in (buf[cur], sw).
+template <int NTP, int W>
+PAI_DEV void pe_finish_p(const DPowEnv<NTP>& E, const PEncC<NTP>& C, int cur, int sw) {
+  const DigitEnv& dc = C.P.dc;
+  const int oth = cur ^ 1;
+  const DNum x = dview<NTP>(E.buf[cur], sw);
+  dmul<NTP>(half_lo<NTP>(E.buf[oth]), half_hi<NTP>(E.buf[oth]), x.d0, x.d1, dc.ONE, dtbl_entry<NTP>(E, 1 << W).d0, &dc);
+  digits_to_plain<NTP>(E.buf[cur], dview<NTP>(E.buf[oth], 1), dc.N);
+  big_copy<2 * NTP>(dtbl_entry<NTP>(E, (1 << W) + 1).d0, E.buf[cur]);
+}
+// Side q and the CRT: h = (omega_q * (1, t_q) - c_p) * p^-2 mod q^2, c = c_p + p^2 * h (4*NTP tiles, buf[0] and buf[1]
+// read as one operand: the two buffers of a thread are adjacent in the interleaved layout).
+template <int NTP, int W>
+PAI_DEV void pe_finish_q(const DPowEnv<NTP>& E, const PEncC<NTP>& C, int cur, int sw, uint32_t* out_row, bool store) {
+  const DigitEnv& dc = C.Q.dc;
+  const int oth = cur ^ 1;
+  const Opnd cp = dtbl_entry<NTP>(E, (1 << W) + 1).d0;                    // c_p = cp_lo + cp_hi * R
+  const Opnd cp_hi{cp.p + (size_t)(2 * NTP) * cp.s, cp.s};
+  DNum x = dview<NTP>(E.buf[cur], sw);
+  dmul<NTP>(half_lo<NTP>(E.buf[oth]), half_hi<NTP>(E.buf[oth]), x.d0, x.d1, C.K1.d0, C.K1.d1, &dc);        // omega_q p^-2 R
+  x = dview<NTP>(E.buf[oth], 1);
+  dmul<NTP>(half_lo<NTP>(E.buf[cur]), half_hi<NTP>(E.buf[cur]), x.d0, x.d1, dc.ONE, dtbl_entry<NTP>(E, 1 << W).d1, &dc);   // c_q p^-2
+  dmul<NTP>(half_lo<NTP>(E.buf[oth]), half_hi<NTP>(E.buf[oth]), cp, dc.ZERO, C.K1N.d0, C.K1N.d1, &dc);      // -cp_lo p^-2
+  dadd<NTP>(dview<NTP>(E.buf[cur], 1), dview<NTP>(E.buf[oth], 1), dc.N);
+  dmul<NTP>(half_lo<NTP>(E.buf[oth]), half_hi<NTP>(E.buf[oth]), cp_hi, dc.ZERO, C.K2N.d0, C.K2N.d1, &dc);   // -cp_hi R p^-2
+  dadd<NTP>(dview<NTP>(E.buf[cur], 1), dview<NTP>(E.buf[oth], 1), dc.N);                                   // h, digits
+  const Opnd h = dtbl_entry<NTP>(E, 0).d0;
+  digits_to_plain<NTP>(E.buf[oth], dview<NTP>(E.buf[cur], 1), dc.N);
+  big_copy<2 * NTP>(h, E.buf[oth]);
+  big_mul<2 * NTP, 2 * NTP, 4 * NTP>(E.buf[0], h, C.P2, 0u);
+  uint32_t cy = 0;
+  for (int t = 0; t < 4 * NTP; t++) {
+    uint32_t a[8], b[8], r[8];
+    ld_tile(E.buf[0], t, a);
+    if (t < 2 * NTP) ld_tile(cp, t, b);
+    else { PAI_UNROLL for (int i = 0; i < 8; i++) b[i] = 0; }
+    cy = add8c(r, a, b, cy);
+    st_tile(E.buf[0], t, r);
+  }
+  if (store) store_row(out_row, E.buf[0], 8 * NTP);
+}
+
+// One ciphertext.  pre_p / pre_q (plain rows r^n mod x^2 computed by the warp kernels) replace the two exponentiations.
+template <int NTP, int W>
+PAI_DEV void prog_priv_encrypt_digit(DPowEnv<NTP>& E, PEncC<NTP>& C, const uint32_t* m_row, const uint32_t* r_row,
+                                     const uint32_t* pre_p, const uint32_t* pre_q, uint32_t* out_row, bool store) {
+  const DNum tpq = dtbl_entry<NTP>(E, 1 << W);                            // [t_p | t_q]
+  pe_msg_digit<NTP>(half_lo<NTP>(E.buf[0]), half_hi<NTP>(E.buf[0]), C.P, m_row);
+  big_copy<NTP>(tpq.d0, half_lo<NTP>(E.buf[0]));
+  pe_msg_digit<NTP>(half_lo<NTP>(E.buf[0]), half_hi<NTP>(E.buf[0]), C.Q, m_row);
+  big_copy<NTP>(tpq.d1, half_lo<NTP>(E.buf[0]));
+  PESideC<NTP>* sides[2] = {&C.P, &C.Q};
+  const uint32_t* pre[2] = {pre_p, pre_q};
+  for (int i = 0; i < 2; i++) {
+    int cur = 0, sw = 1;
+    if (pre[i]) {
+      E.dc = &sides[i]->dc;
+      digit_enter<NTP>(E, pre[i]);
+    } else {
+      cur = pe_pow_side<NTP, W>(E, *sides[i], r_row, &sw);
+    }
+    if (i == 0) pe_finish_p<NTP, W>(E, C, cur, sw);
+    else pe_finish_q<NTP, W>(E, C, cur, sw, out_row, store);
+  }
+}
+
+
+// ------------------------------------------------------------------------------------------------
 // Entering and leaving the digit-Montgomery domain of n^2 for a plain ciphertext row (2*NTH tiles = c_0 + c_1*R).
 // Entry: c*R = dmul((c_0, 0), RR) + dmul((c_1, 0), E3), left in buf[0] as [d1 | d0] (swapped = 1); uses both buffers.
 template <int NTH>

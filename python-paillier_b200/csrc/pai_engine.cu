@@ -11,6 +11,7 @@
 
 #include <algorithm>
 #include <cstdio>
+#include <deque>
 #include <map>
 #include <mutex>
 #include <new>
@@ -248,6 +249,16 @@ struct DecDigitBody {
   int nwin_p, nwin_q; const uint32_t* c; uint32_t* out; long batch; u4* tbl; unsigned long long* counter;
   PAI_MEM void run(u4* smem, const CtaId& id) const { cta_decrypt_digit<NTP, W>(smem, id, nwin_p, nwin_q, c, out, batch, tbl, counter); }
 };
+template <int NTP, int W>
+struct PrivEncDigitBody {
+  const uint32_t* consts; int const_quads;
+  int nwin_p, nwin_q; const uint32_t* m; const uint32_t* r;
+  const uint32_t* pre_p; const uint32_t* pre_q;      // r^n mod p^2, r^n mod q^2 already computed (warp kernels), or null
+  uint32_t* out; long batch; u4* tbl;
+  PAI_MEM void run(u4* smem, const CtaId& id) const {
+    cta_priv_encrypt_digit<NTP, W>(smem, id, nwin_p, nwin_q, m, r, pre_p, pre_q, out, batch, tbl);
+  }
+};
 // one CRT half with h = 1 (used once per key to derive hp / hq): out = L(g^(x-1) mod x^2) mod x
 template <int NTP, int W>
 struct LBody {
@@ -358,6 +369,26 @@ limbs_t padded(const uint32_t* a, int n, int total) {
   for (int i = 0; i < n && i < total; i++) r[i] = a[i];
   return r;
 }
+// a = quo * m + rem (m > 0) by binary long division with one masked subtraction per bit: the operands are key material
+void h_divmod(const limbs_t& a, const limbs_t& m, limbs_t* quo, limbs_t* rem) {
+  const size_t L = m.size() + 1;
+  limbs_t r(L, 0), t(L, 0);
+  if (quo) quo->assign(a.size(), 0);
+  for (long i = 32 * (long)a.size() - 1; i >= 0; i--) {
+    uint32_t c = (a[i >> 5] >> (i & 31)) & 1u;
+    for (size_t j = 0; j < L; j++) { uint32_t v = r[j]; r[j] = (v << 1) | c; c = v >> 31; }
+    uint64_t bo = 0;
+    for (size_t j = 0; j < L; j++) { uint64_t d = (uint64_t)r[j] - (j < m.size() ? m[j] : 0u) - bo; t[j] = (uint32_t)d; bo = (d >> 63) & 1; }
+    const uint32_t keep = 0u - (uint32_t)bo;                 // r < m: r stays
+    for (size_t j = 0; j < L; j++) r[j] = (r[j] & keep) | (t[j] & ~keep);
+    if (quo) (*quo)[i >> 5] |= (uint32_t)(1 - bo) << (i & 31);
+  }
+  if (rem) { *rem = r; rem->resize(m.size()); }
+  std::fill(r.begin(), r.end(), 0);
+  std::fill(t.begin(), t.end(), 0);
+}
+limbs_t h_mod(const limbs_t& a, const limbs_t& m) { limbs_t r; h_divmod(a, m, nullptr, &r); return r; }
+limbs_t h_shl_limbs(const limbs_t& a, int k) { limbs_t r(k, 0); r.insert(r.end(), a.begin(), a.end()); return r; }
 
 // Sliding-window program of a public exponent (see mont_pow_prog): left-to-right, windows of at most w
 // bits that start and end on a 1 bit.  entry = (nsq << 16) | idx, idx = (window value - 1) / 2 or 0xffff.
@@ -556,6 +587,12 @@ struct pai_priv {
   std::recursive_mutex mu;
   long wave = 0;                    // ciphertexts per wave of the throughput decrypt kernel (lazily measured)
   DevBuf<uint32_t> d_coop_e;        // [ p - 1 | q - 1 ] (8*NTP limbs each) for the warp-per-ciphertext path
+  // encryption with the private key (pai_priv_encrypt), built on its first call:
+  DevBuf<uint32_t> d_pe_consts;     // pe_const_limbs<NTP>() limbs (pai_digit.cuh)
+  DevBuf<uint32_t> d_pe_coop_e;     // [ n mod p(p-1) | n mod q(q-1) ] (16*NTP limbs each) for its warp-per-ciphertext route
+  int pe_nwin_p = 0, pe_nwin_q = 0, pe_coop_nwin[2] = {0, 0};
+  long pe_wave = 0;                 // rows per wave of its throughput kernel (routing only)
+  DevBuf<> h_r;                     // staging of pai_priv_encrypt_host (with h_m and h_c, under `mu`)
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -1039,6 +1076,82 @@ int do_priv_digit_setup(pai_priv* k, rt_stream s) {
   return rc;
 }
 
+// ---- encryption with the private key
+template <int NTP>
+Shape priv_enc_shape() { return {2 * NTP, pe_const_limbs<NTP>() / 4, 2, pe_slots(W_DEC)}; }
+template <int NTP>
+int do_priv_encrypt_digit(pai_priv* k, const uint32_t* m, const uint32_t* r, uint32_t* c, long batch, rt_stream s,
+                          const uint32_t* pre_p, const uint32_t* pre_q) {
+  typedef PrivEncDigitBody<NTP, W_DEC> B;
+  const Shape sh = priv_enc_shape<NTP>();
+  return launch_persistent<B>(k->device, k->ws.get(s), sh, batch, s, [&](u4* tbl, unsigned long long*) {
+    return B{k->d_pe_consts.p, sh.cq, k->pe_nwin_p, k->pe_nwin_q, m, r, pre_p, pre_q, c, batch, tbl};
+  });
+}
+// The constants of pai_priv_encrypt (pai_digit.cuh), derived on the host from p, q and p^-1 mod q and uploaded once; the
+// digit blobs of p and q are copied from pd / qd.
+// Host scratch for the key-derived values: every result of a helper is moved into it (never copied, never dropped as a
+// temporary), so each intermediate of the derivation lives in exactly one buffer, and every buffer is zeroed on exit.
+// (h_divmod zeroes its own working rows.)
+struct KeyScratch {
+  std::deque<limbs_t> v;
+  limbs_t& operator()(limbs_t x) { v.push_back(std::move(x)); return v.back(); }
+  ~KeyScratch() { for (limbs_t& x : v) std::fill(x.begin(), x.end(), 0); }
+};
+template <int NTP>
+int do_priv_enc_setup(pai_priv* k, rt_stream s) {
+  const int L1 = 8 * NTP, L2 = 16 * NTP, side = pe_side_limbs<NTP>();
+  KeyScratch S;
+  const limbs_t* x[2] = {&S(padded(k->h_p.data(), L1, L1)), &S(padded(k->h_q.data(), L1, L1))};
+  const limbs_t* x2[2] = {&S(h_mul(*x[0], *x[0])), &S(h_mul(*x[1], *x[1]))};
+  const limbs_t& n = S(h_mul(*x[0], *x[1]));
+  limbs_t& img = S(limbs_t(2 * side + 4 * L2, 0));
+  limbs_t& coop_e = S(limbs_t(2 * L2, 0));
+  auto put = [](const limbs_t& v, uint32_t* o, size_t limbs) { std::copy(v.begin(), v.begin() + limbs, o); };
+  for (int i = 0; i < 2; i++) {                                   // [ yR | yR2 | e1 ] after the digit blob of x
+    const limbs_t& y = *x[i ^ 1];
+    const limbs_t& xm1 = S(h_sub_small(*x[i], 1));
+    const limbs_t& xx1 = S(h_mul(*x[i], xm1));
+    uint32_t* o = img.data() + (size_t)i * side + dc_limbs(NTP);
+    put(S(h_mod(S(h_shl_limbs(y, L1)), *x[i])), o, L1);
+    put(S(h_mod(S(h_shl_limbs(y, 2 * L1)), *x[i])), o + L1, L1);
+    put(S(h_mod(y, xm1)), o + 2 * L1, L1);
+    put(S(h_mod(n, xx1)), coop_e.data() + (size_t)i * L2, L2);
+    k->pe_coop_nwin[i] = (bit_length(xx1) + COOP_W - 1) / COOP_W;
+  }
+  k->pe_nwin_p = (bit_length(*x[0]) + W_DEC - 1) / W_DEC;
+  k->pe_nwin_q = (bit_length(*x[1]) + W_DEC - 1) / W_DEC;
+  // u = p^-2 mod q^2 by one Newton step from (p^-1 mod q)^2 mod q: u = u0 * (2 - p^2 u0) mod q^2
+  const limbs_t& q = *x[1];
+  const limbs_t& q2 = *x2[1];
+  const limbs_t& u0 = S(h_mod(S(h_mul(k->h_pinv, k->h_pinv)), q));
+  const limbs_t& t = S(h_mod(S(h_mul(*x2[0], u0)), q2));
+  const limbs_t& s2 = S(h_mod(S(h_sub(S(h_add_small(S(padded(q2.data(), (int)q2.size(), (int)q2.size() + 1)), 2)), t)), q2));
+  const limbs_t& u = S(h_mod(S(h_mul(u0, s2)), q2));
+  const limbs_t& uR = S(h_mod(S(h_shl_limbs(u, L1)), q2));
+  const limbs_t& uR2 = S(h_mod(S(h_shl_limbs(u, 2 * L1)), q2));
+  const limbs_t* kv[3] = {&uR, &S(h_mod(S(h_sub(q2, uR)), q2)), &S(h_mod(S(h_sub(q2, uR2)), q2))};
+  for (int j = 0; j < 3; j++) {                                   // K1 = u R, K1N = -u R, K2N = -u R^2 as digits base q
+    limbs_t& d0 = S(limbs_t());
+    limbs_t& d1 = S(limbs_t());
+    h_divmod(*kv[j], q, &d1, &d0);
+    uint32_t* o = img.data() + 2 * (size_t)side + (size_t)j * L2;
+    put(d0, o, L1);
+    put(d1, o + L1, L1);
+  }
+  put(*x2[0], img.data() + 2 * (size_t)side + 3 * L2, L2);
+  int rc = k->d_pe_consts.ensure(img.size() * 4);
+  if (!rc) rc = k->d_pe_coop_e.ensure(coop_e.size() * 4);
+  if (!rc) rc = rt_h2d(k->d_pe_consts.p, img.data(), img.size() * 4, s);
+  pai_mod* md[2] = {k->pd, k->qd};
+  for (int i = 0; i < 2 && !rc; i++) rc = rt_d2d(k->d_pe_consts.p + (size_t)i * side, md[i]->d_blob.p, (size_t)dc_limbs(NTP) * 4, s);
+  if (!rc) rc = rt_h2d(k->d_pe_coop_e.p, coop_e.data(), coop_e.size() * 4, s);
+  if (!rc) rc = rt_sync(s);                                      // the host images are read before they are wiped
+  if (!rc) k->pe_wave = std::max(1L, wave_of<PrivEncDigitBody<NTP, W_DEC>>(k->device, priv_enc_shape<NTP>()));
+  if (rc) { k->d_pe_consts.release(true); k->d_pe_coop_e.release(true); }
+  return rc;
+}
+
 // derive one side's constants on the device.  side layout: [ blob(x^2) | blob(x) | xinv | hM | e ]
 template <int NTP>
 int do_side(pai_priv* k, pai_mod* m2, pai_mod* m1, const limbs_t& x, const limbs_t& g_pad, uint32_t* d_side, int nwin,
@@ -1218,6 +1331,18 @@ static int do_coop_decrypt_pow(pai_priv* k, const uint32_t* d_c, uint32_t* up, u
   b.nwin[0] = (bit_length(h_sub_small(k->h_p, 1)) + COOP_W - 1) / COOP_W;
   b.nwin[1] = (bit_length(h_sub_small(k->h_q, 1)) + COOP_W - 1) / COOP_W;
   b.out[0] = up; b.out[1] = uq; b.base = d_c; b.base_limbs = 2 * L2; b.out_limbs = L2; b.batch = batch;
+  return launch_coop<K>(b, 2 * batch, s);
+}
+// r^n mod p^2 and mod q^2 as r^(n mod x(x-1)) for pai_priv_encrypt (the two sides of a row on two warps)
+template <int K>
+static int do_coop_priv_enc_pow(pai_priv* k, const uint32_t* d_r, uint32_t* up, uint32_t* uq, long batch, rt_stream s) {
+  const int L2 = 16 * k->NTP;
+  CoopPowBody<K> b;
+  b.consts = nullptr; b.const_quads = 0; b.nsides = 2;
+  b.blob[0] = k->p2->d_coop.p; b.blob[1] = k->q2->d_coop.p; b.n0inv[0] = k->p2->coop_n0inv; b.n0inv[1] = k->q2->coop_n0inv;
+  b.e[0] = k->d_pe_coop_e.p; b.e[1] = k->d_pe_coop_e.p + L2; b.e_limbs = L2;
+  b.nwin[0] = k->pe_coop_nwin[0]; b.nwin[1] = k->pe_coop_nwin[1];
+  b.out[0] = up; b.out[1] = uq; b.base = d_r; b.base_limbs = L2; b.out_limbs = L2; b.batch = batch;
   return launch_coop<K>(b, 2 * batch, s);
 }
 
@@ -1740,7 +1865,8 @@ int pai_priv_destroy(pai_priv* k) {
   if (!k) return 0;
   rt_set_device(k->device);
   k->d_consts.release(true); k->d_dconsts.release(true); k->d_tc.release(true); k->d_coop_e.release(true);
-  k->ws.release(true); k->h_c.release(true); k->h_m.release(true);
+  k->d_pe_consts.release(true); k->d_pe_coop_e.release(true);
+  k->ws.release(true); k->h_c.release(true); k->h_m.release(true); k->h_r.release(true);
   for (pai_mod* m : {k->pd, k->qd, k->p2, k->q2, k->p1, k->q1}) mod_free(m, true);
   for (limbs_t* h : {&k->h_p, &k->h_q, &k->h_pinv, &k->h_hp, &k->h_hq}) std::fill(h->begin(), h->end(), 0);
   delete k;
@@ -1806,6 +1932,36 @@ int pai_decrypt(pai_priv* k, const uint32_t* d_c, uint32_t* d_m, long batch, voi
   }
   return decrypt_rows(k, d_c, d_m, batch, (rt_stream)stream);
 }
+int pai_priv_encrypt(pai_priv* k, const uint32_t* d_m, const uint32_t* d_r, uint32_t* d_c, long batch, void* stream) {
+  DeviceGuard device_guard_; (void)device_guard_;
+  if (!k || !d_m || !d_r || !d_c || batch < 0) { g_err = "bad argument"; return PAI_E_ARG; }
+  CtxLock lock_(k->mu);
+  if (batch == 0) return 0;
+  rt_stream s = (rt_stream)stream;
+  int rc = rt_set_device(k->device);
+  if (!rc && !k->d_pe_consts.p) { DISPATCH_NTP(k->NTP, rc = do_priv_enc_setup<NTP>(k, s)); }
+  if (rc) return rc;
+  const long ncoop = coop_rows(batch, k->pe_wave);
+  if (ncoop) {
+    // both exponentiations on one warp each (pai_coop.cuh), then the message factors and the CRT one thread per row
+    const int L2 = 16 * k->NTP;
+    const long off = batch - ncoop;
+    rc = ensure_coop(k->p2, s);
+    if (!rc) rc = ensure_coop(k->q2, s);
+    StreamWs& w = k->ws.get(s);
+    if (!rc) rc = w.coop_u.ensure((size_t)2 * ncoop * L2 * 4);
+    if (rc) return rc;
+    uint32_t* up = (uint32_t*)w.coop_u.p;
+    uint32_t* uq = up + (size_t)ncoop * L2;
+    DISPATCH_K(k->p2->coopK, rc = do_coop_priv_enc_pow<K>(k, d_r + off * L2, up, uq, ncoop, s));
+    if (rc) return rc;
+    DISPATCH_NTP(k->NTP, rc = do_priv_encrypt_digit<NTP>(k, d_m + off * L2, d_r + off * L2, d_c + off * 2 * L2, ncoop, s, up, uq));
+    if (rc || off == 0) return rc;
+    batch = off;
+  }
+  DISPATCH_NTP(k->NTP, rc = do_priv_encrypt_digit<NTP>(k, d_m, d_r, d_c, batch, s, nullptr, nullptr));
+  return rc;
+}
 
 // ---------------------------------------------------------------------------------------- host-pointer variants
 
@@ -1832,6 +1988,12 @@ int pai_decrypt_host(pai_priv* k, const uint32_t* c, uint32_t* m, long batch) {
   const size_t bn = (size_t)batch * 16 * k->NTP * 4;
   return run_staged(k->mu, k->device, batch, {{k->h_c, c, 2 * bn}}, {{k->h_m, m, bn}},
                     [&] { return pai_decrypt(k, dev(k->h_c), dev(k->h_m), batch, nullptr); });
+}
+int pai_priv_encrypt_host(pai_priv* k, const uint32_t* m, const uint32_t* r, uint32_t* c, long batch) {
+  if (!k || !m || !r || !c || batch < 0) { g_err = "bad argument"; return PAI_E_ARG; }
+  const size_t bn = (size_t)batch * 16 * k->NTP * 4;
+  return run_staged(k->mu, k->device, batch, {{k->h_m, m, bn}, {k->h_r, r, bn}}, {{k->h_c, c, 2 * bn}},
+                    [&] { return pai_priv_encrypt(k, dev(k->h_m), dev(k->h_r), dev(k->h_c), batch, nullptr); });
 }
 int pai_mod_mulmod_host(pai_mod* m, const uint32_t* a, const uint32_t* b, uint32_t* out, long batch) {
   if (!m || !a || !b || !out || batch < 0) { g_err = "bad argument"; return PAI_E_ARG; }

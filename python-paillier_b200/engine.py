@@ -74,10 +74,12 @@ SYMBOLS = {
     "pai_priv_c_limbs": (ctypes.c_int, [_vp]),
     "pai_priv_get": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp]),
     "pai_decrypt": (ctypes.c_int, [_vp, _vp, _vp, ctypes.c_long, _vp]),
+    "pai_priv_encrypt": (ctypes.c_int, [_vp, _vp, _vp, _vp, ctypes.c_long, _vp]),
     "pai_encrypt_host": (ctypes.c_int, [_vp, _vp, _vp, _vp, ctypes.c_long]),
     "pai_raw_add_host": (ctypes.c_int, [_vp, _vp, _vp, _vp, ctypes.c_long]),
     "pai_raw_mul_host": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, ctypes.c_long]),
     "pai_decrypt_host": (ctypes.c_int, [_vp, _vp, _vp, ctypes.c_long]),
+    "pai_priv_encrypt_host": (ctypes.c_int, [_vp, _vp, _vp, _vp, ctypes.c_long]),
     "pai_mod_mulmod_host": (ctypes.c_int, [_vp, _vp, _vp, _vp, ctypes.c_long]),
     "pai_mod_powmod_host": (ctypes.c_int, [_vp, _vp, ctypes.c_int, _vp, ctypes.c_int, ctypes.c_int, _vp, ctypes.c_long]),
     "pai_mod_invert_host": (ctypes.c_int, [_vp, _vp, ctypes.c_int, _vp, _vp, ctypes.c_long]),
@@ -267,6 +269,23 @@ def _pipeline(ranges, pack, run, unpack):
     return out
 
 
+def _raw_encrypt_pipelined(ctx, plaintexts, r_values):
+    """raw_encrypt of Python ints through ctx.encrypt_host (a public or a private context): m of any sign or size (reduced
+    mod n as the reference's ``% nsquare`` does, phe/paillier.py:134), r in [1, n)."""
+    n = ctx.n
+    lim = 1 << (32 * ctx.n_limbs)
+    count = len(plaintexts)
+    if len(r_values) != count:
+        raise ValueError("plaintexts and r_values differ in length")
+
+    def pack(lo, hi):
+        return (ints_to_limbs([p if 0 <= p < lim else p % n for p in plaintexts[lo:hi]], ctx.n_limbs),
+                ints_to_limbs(r_values[lo:hi], ctx.n_limbs))
+    if count < _PIPE_MIN:
+        return limbs_to_ints(ctx.encrypt_host(*pack(0, count)))
+    return _pipeline(_chunk_ranges(count, ctx.wave()), pack, lambda a: ctx.encrypt_host(*a), limbs_to_ints)
+
+
 # ---------------------------------------------------------------------------- contexts
 class ModContext:
     """Montgomery context of one odd modulus: batched powmod / mulmod / invert (the phe/util.py seam)."""
@@ -430,18 +449,7 @@ class PublicContext:
     def raw_encrypt(self, plaintexts, r_values):
         """[(1 + n*m) * r^n mod n^2]  for ints m (any sign/size: reduced mod n as the reference's
         ``% nsquare`` does, phe/paillier.py:134) and r in [1, n)."""
-        n = self.n
-        lim = 1 << (32 * self.n_limbs)
-        count = len(plaintexts)
-        if len(r_values) != count:
-            raise ValueError("plaintexts and r_values differ in length")
-
-        def pack(lo, hi):
-            return (ints_to_limbs([p if 0 <= p < lim else p % n for p in plaintexts[lo:hi]], self.n_limbs),
-                    ints_to_limbs(r_values[lo:hi], self.n_limbs))
-        if count < _PIPE_MIN:
-            return limbs_to_ints(self.encrypt_host(*pack(0, count)))
-        return _pipeline(_chunk_ranges(count, self.wave()), pack, lambda a: self.encrypt_host(*a), limbs_to_ints)
+        return _raw_encrypt_pipelined(self, plaintexts, r_values)
 
     def wave(self):
         """Rows per full wave of the throughput encrypt kernel (batches that are multiples of it waste nothing)."""
@@ -460,7 +468,8 @@ class PublicContext:
 
 
 class PrivateContext:
-    """Engine context of a private key (p, q): batched raw_decrypt (CRT)."""
+    """Engine context of a private key (p, q): batched raw_decrypt (CRT), and raw_encrypt through the CRT with the same
+    bits as PublicContext's."""
 
     def __init__(self, p, q, device=0, engine=None):
         self.eng = engine or get_engine()
@@ -499,6 +508,20 @@ class PrivateContext:
         out = np.empty((c.shape[0], self.n_limbs), dtype=np.uint32)
         self.eng.check(self.eng.lib.pai_decrypt_host(self.h, _ptr(c), _ptr(out), c.shape[0]))
         return out
+
+    def encrypt_dev(self, d_m, d_r, d_c, batch, stream=None):
+        """d_c = (1 + n*d_m) * d_r^n mod n^2 with the private key (pai_priv_encrypt): the bits PublicContext.encrypt_dev
+        gives for the same rows.  Rows of n_limbs / c_limbs columns (this context's layout)."""
+        self.eng.check(self.eng.lib.pai_priv_encrypt(self.h, _ptr(d_m), _ptr(d_r), _ptr(d_c), batch, _ptr(stream)))
+
+    def encrypt_host(self, m, r):
+        out = np.empty((m.shape[0], self.c_limbs), dtype=np.uint32)
+        self.eng.check(self.eng.lib.pai_priv_encrypt_host(self.h, _ptr(m), _ptr(r), _ptr(out), m.shape[0]))
+        return out
+
+    def raw_encrypt(self, plaintexts, r_values):
+        """As PublicContext.raw_encrypt, computed with the private key."""
+        return _raw_encrypt_pipelined(self, plaintexts, r_values)
 
     def raw_decrypt(self, ciphertexts):
         """raw_decrypt for ints of any size/sign (reduced mod n^2 first; the reference's powmod

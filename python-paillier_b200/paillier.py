@@ -103,6 +103,11 @@ class PaillierPublicKey(object):
 
     def raw_encrypt_batch(self, plaintexts, r_values=None):
         """Batched raw_encrypt: list of ints -> list of ints (one kernel launch)."""
+        return self._raw_encrypt_batch(plaintexts, r_values, self.engine_context())
+
+    def _raw_encrypt_batch(self, plaintexts, r_values, ctx):
+        """raw_encrypt_batch on the engine context `ctx`: this key's PublicContext or its private key's PrivateContext,
+        which give the same bits."""
         plaintexts = list(plaintexts)
         for m in plaintexts:
             if not isinstance(m, int):
@@ -122,9 +127,9 @@ class PaillierPublicKey(object):
         r_values = [r if 0 < r < self.nsquare else r % self.nsquare for r in r_values]
         wide = {i: self.raw_encrypt(plaintexts[i], r) for i, r in enumerate(r_values) if r >= lim}
         if not wide:
-            return self.engine_context().raw_encrypt(plaintexts, r_values)
+            return ctx.raw_encrypt(plaintexts, r_values)
         keep = [i for i in range(len(plaintexts)) if i not in wide]
-        bulk = iter(self.engine_context().raw_encrypt([plaintexts[i] for i in keep], [r_values[i] for i in keep]))
+        bulk = iter(ctx.raw_encrypt([plaintexts[i] for i in keep], [r_values[i] for i in keep]))
         return [wide[i] if i in wide else next(bulk) for i in range(len(plaintexts))]
 
     def encrypt(self, value, precision=None, r_value=None):
@@ -211,6 +216,15 @@ class PaillierPrivateKey(object):
         if not isinstance(ciphertext, int):
             raise TypeError('Expected ciphertext to be an int, not: %s' % type(ciphertext))
         return self.engine_context().raw_decrypt([ciphertext])[0]
+
+    def raw_encrypt_batch(self, plaintexts, r_values=None):
+        """public_key.raw_encrypt_batch element by element, computed with p and q (pai_priv_encrypt)."""
+        return self.public_key._raw_encrypt_batch(plaintexts, r_values, self.engine_context())
+
+    def encrypt_batch(self, values, precision=None, r_values=None):
+        """public_key.encrypt_batch (same ciphertexts and exponents for the same r_values), computed with p and q."""
+        from .vector import EncryptedVector
+        return EncryptedVector.encrypt(self.public_key, values, precision=precision, r_values=r_values, private_key=self)
 
     def raw_decrypt_batch(self, ciphertexts):
         for c in ciphertexts:

@@ -316,22 +316,24 @@ class EncryptedVector(object):
 
     # ------------------------------------------------------------------ construction
     @classmethod
-    def encrypt(cls, public_key, values, precision=None, r_values=None):
+    def encrypt(cls, public_key, values, precision=None, r_values=None, private_key=None):
         """Encode every value (EncodedNumber.encode) and encrypt the batch in one launch.  With
-        r_values None each element gets a fresh random r and is therefore already obfuscated."""
+        r_values None each element gets a fresh random r and is therefore already obfuscated.  With the private key
+        given, the encryption runs through the CRT (pai_priv_encrypt) and gives the same ciphertexts."""
         if len(values) and any(isinstance(v, EncodedNumber) for v in (values if not isinstance(values, np.ndarray) else [])):
             encs = [v if isinstance(v, EncodedNumber) else EncodedNumber.encode(public_key, v, precision) for v in values]
-            return cls.encrypt_encoded(public_key, [e.encoding for e in encs], [e.exponent for e in encs], r_values)
+            return cls.encrypt_encoded(public_key, [e.encoding for e in encs], [e.exponent for e in encs], r_values, private_key)
         limbs, exps = encode_batch(public_key, values, precision)
-        return cls._encrypt_limbs(public_key, limbs, exps, r_values)
+        return cls._encrypt_limbs(public_key, limbs, exps, r_values, private_key)
 
     @classmethod
-    def encrypt_encoded(cls, public_key, encodings, exponents, r_values=None):
+    def encrypt_encoded(cls, public_key, encodings, exponents, r_values=None, private_key=None):
         ctx = public_key.engine_context()
-        return cls._encrypt_limbs(public_key, ints_to_limbs([e % public_key.n for e in encodings], ctx.n_limbs), exponents, r_values)
+        return cls._encrypt_limbs(public_key, ints_to_limbs([e % public_key.n for e in encodings], ctx.n_limbs), exponents, r_values,
+                                  private_key)
 
     @classmethod
-    def _encrypt_limbs(cls, public_key, m_limbs, exponents, r_values=None):
+    def _encrypt_limbs(cls, public_key, m_limbs, exponents, r_values=None, private_key=None):
         ctx = public_key.engine_context()
         count = int(m_limbs.shape[0])
         obf = r_values is None
@@ -344,6 +346,13 @@ class EncryptedVector(object):
                 ctx.random_lt_n_dev(d_r, count, stream=_stream(ctx))
         else:
             d_r = _to_dev(ints_to_limbs(list(r_values), ctx.n_limbs), ctx)
+        if private_key is not None:
+            # the private context sizes its rows from max(p, q): re-pad the rows in, trim the all-zero columns out
+            pctx = private_key.engine_context()
+            d_c = torch.empty((count, pctx.c_limbs), dtype=torch.int32, device=d_m.device)
+            if count:
+                pctx.encrypt_dev(_rows_for(pctx.n_limbs, d_m), _rows_for(pctx.n_limbs, d_r), d_c, count, stream=_stream(pctx))
+            return cls(public_key, _rows_for(ctx.c_limbs, d_c), exponents, obfuscated=obf)
         d_c = torch.empty((count, ctx.c_limbs), dtype=torch.int32, device=d_m.device)
         if count:
             ctx.encrypt_dev(d_m, d_r, d_c, count, stream=_stream(ctx))
