@@ -175,6 +175,21 @@ int pai_limbs_to_decimal(const uint32_t* d_limbs, int limbs, uint8_t* d_text, lo
 int pai_decimal_to_limbs(const uint8_t* d_text, int width, uint32_t* d_limbs, int limbs, int32_t* d_status, long batch, int device,
                          void* stream);
 
+/* ---- packed fixed-point plaintexts: many signed values per ciphertext --------------------------------------
+ * No reference counterpart (BatchCrypt-style packing; DESIGN.md §3.10).  A plaintext row holds K = (bits(n) - 1) / slot_bits
+ * signed slots s_j with |s_j| <= 2^(slot_bits-1) - 1 as P = sum_j s_j * 2^(slot_bits*j), stored as P mod n.  Then
+ * |P| < 2^(bits(n)-2) < n/2, and raw_add / raw_mul by an integer act on every slot while the slots stay within that bound.  Slot j of row r
+ * is value r*K + j of a flat int64 array.  Asynchronous on `stream`; no workspace. */
+/* K for this key, or PAI_E_ARG for slot_bits outside 2..63 or when not even one slot fits */
+int pai_pack_slots_per_row(const pai_pub* k, int slot_bits);
+/* m[r] = (sum_j s[r*K + j] * 2^(slot_bits*j)) mod n for r < ceil(count / K), missing slots 0.  d_status[r] = 1 where a slot
+ * of row r is outside (-2^(slot_bits-1), 2^(slot_bits-1)); that row is zeroed.  m: [rows][pai_pub_n_limbs()]. */
+int pai_pack_slots(pai_pub* k, const int64_t* d_slots, long count, int slot_bits, uint32_t* d_m, int32_t* d_status, void* stream);
+/* inverse: centre-lift mod n (m <= (n-1)/2: P = m, else m - n), balanced base-2^slot_bits digits into the first `count`
+ * slots; d_status[r] = 1 where row r is not a packing (m >= n, a digit -2^(slot_bits-1), or a nonzero part above slot
+ * K-1), its slots are zeroed.  It accepts exactly the rows pai_pack_slots produces. */
+int pai_unpack_slots(pai_pub* k, const uint32_t* d_m, int slot_bits, int64_t* d_slots, long count, int32_t* d_status, void* stream);
+
 /* ---- batched primality testing for key generation ----------------------------------------------------------
  * result[i] = 1 if candidate i passes `rounds` Miller-Rabin rounds with the bases given, 0 if it is composite:
  * util.miller_rabin (phe/util.py:381-417) for a whole batch of candidates, one thread per candidate, each with its own

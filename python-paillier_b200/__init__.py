@@ -11,6 +11,6 @@ from .encoding import EncodedNumber  # noqa: F401,E402
 from .paillier import (DEFAULT_KEYSIZE, EncryptedNumber, PaillierPrivateKey, PaillierPrivateKeyring,  # noqa: F401,E402
                        PaillierPublicKey, generate_paillier_keypair, generate_paillier_keypairs)
 from . import util  # noqa: F401,E402
-from .vector import EncryptedVector  # noqa: F401,E402
+from .vector import EncryptedVector, PackedEncryptedVector  # noqa: F401,E402
 
 __version__ = "0.1.0"

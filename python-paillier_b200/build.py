@@ -12,7 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libpaillier_b200.so")
 SOURCES = ["pai_engine.cu"]
-HEADERS = ["pai_core.cuh", "pai_kernels.cuh", "pai_digit.cuh", "pai_cta.cuh", "pai_coop.cuh", "pai_tc.cuh", "pai_rng.cuh", "pai_radix.cuh", "pai_rt.h", os.path.join("..", "..", "include", "paillier_b200.h")]
+HEADERS = ["pai_core.cuh", "pai_kernels.cuh", "pai_digit.cuh", "pai_cta.cuh", "pai_coop.cuh", "pai_tc.cuh", "pai_rng.cuh", "pai_radix.cuh", "pai_pack.cuh", "pai_rt.h", os.path.join("..", "..", "include", "paillier_b200.h")]
 # --split-compile 0: the device optimisation of the many kernel instantiations runs on every host core
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "--split-compile", "0",
               "-Xcompiler", "-fPIC", "-shared", "-Xptxas", "-v"]

@@ -8,6 +8,7 @@
 // host side only pads limb arrays, multiplies p*q / n*n once per key (schoolbook, a few thousand
 // word operations), sizes launches and workspaces, and sequences kernels on the caller's stream.
 #include "pai_rt.h"
+#include "pai_pack.cuh"
 
 #include <algorithm>
 #include <cstdio>
@@ -224,6 +225,27 @@ struct FromDecBody {
     for (long g = (long)id.cta * id.nthr + id.tid; g < batch; g += (long)id.ncta * id.nthr) {
       int st = radix_from_decimal((uint32_t*)smem, id.tid, id.nthr, text + g * (long)width, width, limbs + g * L, L);
       if (status) status[g] = st;
+    }
+  }
+};
+// packed fixed-point rows (pai_pack.cuh), one thread per plaintext row; n (ln limbs) is the CTA's constant area
+struct PackBody {
+  const uint32_t* consts; int const_quads;
+  const int64_t* s; long count; int b, K, ln; uint32_t* m; int32_t* status; long rows;
+  PAI_MEM void run(u4* smem, const CtaId& id) const {
+    for (long r = (long)id.cta * id.nthr + id.tid; r < rows; r += (long)id.ncta * id.nthr) {
+      const long lo = r * K;
+      status[r] = pack_row(s + lo, count - lo < K ? (int)(count - lo) : K, b, (const uint32_t*)smem, ln, m + r * ln);
+    }
+  }
+};
+struct UnpackBody {
+  const uint32_t* consts; int const_quads;
+  const uint32_t* m; int b, K, ln; int64_t* s; long count; int32_t* status; long rows;
+  PAI_MEM void run(u4* smem, const CtaId& id) const {
+    for (long r = (long)id.cta * id.nthr + id.tid; r < rows; r += (long)id.ncta * id.nthr) {
+      const long lo = r * K;
+      status[r] = unpack_row(m + r * ln, (const uint32_t*)smem, ln, b, K, s + lo, count - lo < K ? (int)(count - lo) : K);
     }
   }
 };
@@ -1446,6 +1468,24 @@ int run_staged(std::recursive_mutex& mu, int device, long batch, std::initialize
 }
 template <class T = uint32_t>
 T* dev(const DevBuf<>& b) { return (T*)b.p; }
+
+// pai_pack_slots / pai_unpack_slots: one launch of `b` over the rows of `count` slots, 128 threads per CTA, n in shared
+// memory; no workspace, so no lock
+template <class Body>
+int pack_launch(pai_pub* k, const void* d_in, void* d_out, int32_t* d_status, long count, int slot_bits, void* stream, Body b) {
+  DeviceGuard device_guard_; (void)device_guard_;
+  const int K = pai_pack_slots_per_row(k, slot_bits);
+  if (K < 0) return K;
+  if (!d_in || !d_out || !d_status || count < 0) { g_err = "bad argument"; return PAI_E_ARG; }
+  if (count == 0) return 0;
+  int rc = rt_set_device(k->nsq->device);
+  if (rc) return rc;
+  const long rows = (count + K - 1) / K;
+  b.consts = k->d_nth; b.const_quads = k->ln / 4;
+  b.b = slot_bits; b.K = K; b.ln = k->ln; b.count = count; b.status = d_status; b.rows = rows;
+  const long blocks = (rows + 127) / 128;
+  return rt_launch(b, (int)std::min(blocks, (long)rt_sm_count(k->nsq->device) * 16), 128, (size_t)k->ln * 4, (rt_stream)stream);
+}
 }  // namespace
 
 extern "C" {
@@ -1696,6 +1736,23 @@ int pai_decimal_to_limbs(const uint8_t* d_text, int width, uint32_t* d_limbs, in
   if ((rc = radix_geometry(device, limbs, batch, &grid, &nthr, &smem))) return rc;
   FromDecBody b{nullptr, 0, d_text, width, d_limbs, limbs, d_status, batch};
   return rt_launch(b, grid, nthr, smem, (rt_stream)stream);
+}
+// ---- packed fixed-point rows (pai_pack.cuh) ------------------------------------------------------
+int pai_pack_slots_per_row(const pai_pub* k, int slot_bits) {
+  if (!k || slot_bits < 2 || slot_bits > 63) { g_err = "bad argument"; return PAI_E_ARG; }
+  const int K = (bit_length(k->h_n) - 1) / slot_bits;
+  if (K < 1) { g_err = "slot wider than the key"; return PAI_E_ARG; }
+  return K;
+}
+int pai_pack_slots(pai_pub* k, const int64_t* d_slots, long count, int slot_bits, uint32_t* d_m, int32_t* d_status, void* stream) {
+  PackBody b{};
+  b.s = d_slots; b.m = d_m;
+  return pack_launch(k, d_slots, d_m, d_status, count, slot_bits, stream, b);
+}
+int pai_unpack_slots(pai_pub* k, const uint32_t* d_m, int slot_bits, int64_t* d_slots, long count, int32_t* d_status, void* stream) {
+  UnpackBody b{};
+  b.m = d_m; b.s = d_slots;
+  return pack_launch(k, d_m, d_slots, d_status, count, slot_bits, stream, b);
 }
 int pai_raw_add(pai_pub* k, const uint32_t* d_a, const uint32_t* d_b, uint32_t* d_c, long batch, void* stream) {
   DeviceGuard device_guard_; (void)device_guard_;

@@ -60,6 +60,9 @@ SYMBOLS = {
     "pai_decimal_width": (ctypes.c_int, [ctypes.c_int]),
     "pai_limbs_to_decimal": (ctypes.c_int, [_vp, ctypes.c_int, _vp, ctypes.c_long, ctypes.c_int, _vp]),
     "pai_decimal_to_limbs": (ctypes.c_int, [_vp, ctypes.c_int, _vp, ctypes.c_int, _vp, ctypes.c_long, ctypes.c_int, _vp]),
+    "pai_pack_slots_per_row": (ctypes.c_int, [_vp, ctypes.c_int]),
+    "pai_pack_slots": (ctypes.c_int, [_vp, _vp, ctypes.c_long, ctypes.c_int, _vp, _vp, _vp]),
+    "pai_unpack_slots": (ctypes.c_int, [_vp, _vp, ctypes.c_int, _vp, ctypes.c_long, _vp, _vp]),
     "pai_raw_add": (ctypes.c_int, [_vp, _vp, _vp, _vp, ctypes.c_long, _vp]),
     "pai_raw_mul": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, ctypes.c_long, _vp]),
     "pai_miller_rabin": (ctypes.c_int, [_vp, ctypes.c_int, _vp, ctypes.c_int, _vp, ctypes.c_long, ctypes.c_int, _vp]),
@@ -421,6 +424,24 @@ class PublicContext:
         self.eng.check(self.eng.lib.pai_raw_matvec(self.h, _ptr(d_c), ncols, _ptr(d_indptr), _ptr(d_indices), _ptr(d_mag),
                                                    mag_limbs, mag_bits, _ptr(d_neg), nnz, nrows, _ptr(d_out),
                                                    _ptr(d_status), _ptr(stream)))
+
+    def slots_per_row(self, slot_bits):
+        """K, the signed slots of `slot_bits` bits one plaintext row of this key holds (pai_pack_slots_per_row)."""
+        k = int(self.eng.lib.pai_pack_slots_per_row(self.h, slot_bits))
+        if k < 0:
+            raise ValueError("%d-bit slots: slot_bits must be 2..63 and at most bits(n) - 1" % slot_bits)
+        return k
+
+    def pack_slots_dev(self, d_slots, count, slot_bits, d_m, d_status, stream=None):
+        """d_m [ceil(count / K), n_limbs] <- the int64 slots d_slots [count] packed K to a row, mod n; d_status [rows] = 1
+        where a slot does not fit (that row is zeroed)."""
+        self.eng.check(self.eng.lib.pai_pack_slots(self.h, _ptr(d_slots), count, slot_bits, _ptr(d_m), _ptr(d_status),
+                                                   _ptr(stream)))
+
+    def unpack_slots_dev(self, d_m, slot_bits, d_slots, count, d_status, stream=None):
+        """Inverse of pack_slots_dev: d_status [rows] = 1 where a row is not a packing (its slots are zeroed)."""
+        self.eng.check(self.eng.lib.pai_unpack_slots(self.h, _ptr(d_m), slot_bits, _ptr(d_slots), count, _ptr(d_status),
+                                                     _ptr(stream)))
 
     def matvec_window(self, ncols, nrows, nnz, bits, with_neg):
         """The window width raw_matvec_dev picks for these shapes."""

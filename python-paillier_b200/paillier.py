@@ -151,6 +151,13 @@ class PaillierPublicKey(object):
         from .vector import EncryptedVector
         return EncryptedVector.encrypt(self, values, precision=precision, r_values=r_values)
 
+    def encrypt_packed(self, values, bound, frac_bits=24, headroom=1024, r_values=None):
+        """Fixed-point values packed many to a ciphertext (PackedEncryptedVector, DESIGN.md section 3.10): |x| <= bound,
+        frac_bits fractional bits, slots wide enough for `headroom` such vectors to be added.  r_values: one per
+        ciphertext, or None for fresh ones."""
+        from .vector import PackedEncryptedVector
+        return PackedEncryptedVector.encrypt(self, values, bound, frac_bits, headroom, r_values)
+
 
 class PaillierPrivateKey(object):
     """Private key (p, q) with CRT decryption (phe/paillier.py:197-380)."""
@@ -226,6 +233,11 @@ class PaillierPrivateKey(object):
         from .vector import EncryptedVector
         return EncryptedVector.encrypt(self.public_key, values, precision=precision, r_values=r_values, private_key=self)
 
+    def encrypt_packed(self, values, bound, frac_bits=24, headroom=1024, r_values=None):
+        """public_key.encrypt_packed (the same ciphertexts for the same r_values), computed with p and q."""
+        from .vector import PackedEncryptedVector
+        return PackedEncryptedVector.encrypt(self.public_key, values, bound, frac_bits, headroom, r_values, private_key=self)
+
     def raw_decrypt_batch(self, ciphertexts):
         for c in ciphertexts:
             if not isinstance(c, int):
@@ -233,7 +245,7 @@ class PaillierPrivateKey(object):
         return self.engine_context().raw_decrypt(list(ciphertexts))
 
     def decrypt_batch(self, vector):
-        """Decrypt and decode an EncryptedVector -> list of Python numbers."""
+        """Decrypt and decode an EncryptedVector -> list of Python numbers (a PackedEncryptedVector -> float64 tensor)."""
         return vector.decrypt(self)
 
     # the reference exposes these helpers as methods (phe/paillier.py:356-374); kept for API parity

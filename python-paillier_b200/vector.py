@@ -6,6 +6,9 @@ launch per vector operation, ciphertexts stay in HBM as [B, c_limbs] uint32 limb
 only converted to Python ints on request.  Semantics per element are those of EncryptedNumber
 (exponent alignment before add, phe/paillier.py:695-700; lazy obfuscation, :565-566).
 """
+import fractions
+import math
+import numbers
 import operator
 import os
 
@@ -334,11 +337,15 @@ class EncryptedVector(object):
 
     @classmethod
     def _encrypt_limbs(cls, public_key, m_limbs, exponents, r_values=None, private_key=None):
+        return cls._encrypt_dev_rows(public_key, _to_dev(m_limbs, public_key.engine_context()), exponents, r_values, private_key)
+
+    @classmethod
+    def _encrypt_dev_rows(cls, public_key, d_m, exponents, r_values=None, private_key=None):
+        """Encrypt the plaintext rows d_m [B, n_limbs] (int32, on the key's device) in one launch."""
         ctx = public_key.engine_context()
-        count = int(m_limbs.shape[0])
+        count = int(d_m.shape[0])
         obf = r_values is None
         torch = _torch()
-        d_m = _to_dev(m_limbs, ctx)
         if r_values is None:
             # fresh obfuscators drawn on the device from a ChaCha20 stream keyed by os.urandom (pai_rng.cuh)
             d_r = torch.empty((count, ctx.n_limbs), dtype=torch.int32, device=d_m.device)
@@ -757,11 +764,233 @@ class EncryptedVector(object):
         return decode_batch(self.public_key, self._decrypt_rows(ctx), self.exponents)
 
     def _decrypt_rows(self, ctx):
-        """raw_decrypt of every row -> host uint32 matrix [B, n_limbs of the PUBLIC layout].  The private context sizes
+        """raw_decrypt of every row -> host uint32 matrix [B, n_limbs of the PUBLIC layout]."""
+        return _to_host(self._decrypt_rows_dev(ctx))
+
+    def _decrypt_rows_dev(self, ctx):
+        """raw_decrypt of every row -> device int32 matrix [B, n_limbs of the PUBLIC layout].  The private context sizes
         its rows from max(p, q), the public one from n: for unbalanced primes they differ, and the rows are re-padded."""
         torch = _torch()
         count = len(self)
         d_c = _rows_for(ctx.c_limbs, self.limbs)
         d_m = torch.empty((count, ctx.n_limbs), dtype=torch.int32, device=self.limbs.device)
         ctx.decrypt_dev(d_c, d_m, count, stream=_stream(ctx))
-        return _to_host(_rows_for(self.public_key.engine_context().n_limbs, d_m))
+        return _rows_for(self.public_key.engine_context().n_limbs, d_m)
+
+
+# ------------------------------------------------------------------------------------------------------
+# Packed fixed-point vectors (DESIGN.md §3.10): K signed b-bit slots per plaintext, packed and unpacked on the device.
+def _slot_max(slot_bits):
+    return (1 << (slot_bits - 1)) - 1
+
+
+def _quantise(values, bound, frac_bits, device):
+    """values -> (int64 tensor of round_half_even(x * 2^frac_bits) on `device`, shape).  NaN, inf or |x| > bound raise
+    ValueError.  Float dtypes go through float64 (exact for every float dtype; the scaling by 2^f is exact), integer dtypes
+    take an exact int64 path.  The caller has checked that ceil(bound * 2^f) < 2^62."""
+    torch = _torch()
+    if isinstance(values, torch.Tensor):
+        t = values.detach()
+    else:
+        a = np.asarray(values)
+        if a.dtype.kind == "u" and a.dtype.itemsize == 8:         # torch has no general uint64: range check here
+            if a.size and int(a.max()) > bound:
+                raise ValueError("a value exceeds the declared bound %r" % (bound,))
+            a = a.astype(np.int64)
+        if a.dtype.kind not in "biuf":
+            raise TypeError("values must be real numbers, got dtype %s" % a.dtype)
+        t = torch.as_tensor(a)
+    if t.is_complex():
+        raise TypeError("values must be real numbers, got dtype %s" % t.dtype)
+    shape = tuple(int(x) for x in t.shape)
+    t = t.to(device).reshape(-1)
+    if t.is_floating_point():
+        x = t.to(torch.float64)
+        if not bool(torch.isfinite(x).all().item()):
+            raise ValueError("values must be finite")
+        if bool((x.abs() > float(bound)).any().item()):
+            raise ValueError("a value exceeds the declared bound %r" % (bound,))
+        return torch.round(x * float(2 ** frac_bits)).to(torch.int64).contiguous(), shape
+    x = t.to(torch.int64)
+    ib = min(int(math.floor(bound)), 2 ** 63 - 1)
+    if bool(((x > ib) | (x < -ib)).any().item()):
+        raise ValueError("a value exceeds the declared bound %r" % (bound,))
+    # |x| * 2^f <= ceil(bound * 2^f) < 2^62; for f >= 62 that leaves only x = 0
+    return (x * (1 << frac_bits) if frac_bits < 62 else x).contiguous(), shape
+
+
+class PackedEncryptedVector(object):
+    """Fixed-point values packed many to a ciphertext (DESIGN.md §3.10).
+
+    Each value x is quantised to the integer slot q = round_half_even(x * 2^frac_bits); slots_per_ciphertext slots of
+    slot_bits bits share one plaintext.  Homomorphic addition and multiplication by an integer act on every slot at once.
+    slot_bound is a public bound on every |slot|, derived from the bound declared at encryption, never from the data;
+    an operation whose result could leave 2^(slot_bits-1) - 1 raises OverflowError before anything runs.
+
+    The rows are an EncryptedVector with exponents 0 (``.ciphertexts``); +, * and obfuscate() are its operations."""
+    __array_ufunc__ = None
+
+    def __init__(self, ciphertexts, shape, slot_bits, frac_bits, slot_bound):
+        self.ciphertexts = ciphertexts
+        self.shape = tuple(int(x) for x in shape)
+        self.slot_bits = int(slot_bits)
+        self.frac_bits = int(frac_bits)
+        self.slot_bound = int(slot_bound)
+        self.slots_per_ciphertext = ciphertexts.public_key.engine_context().slots_per_row(self.slot_bits)
+
+    @property
+    def public_key(self):
+        return self.ciphertexts.public_key
+
+    def __len__(self):
+        return math.prod(self.shape)
+
+    # ------------------------------------------------------------------ construction
+    @classmethod
+    def encrypt(cls, public_key, values, bound, frac_bits=24, headroom=1024, r_values=None, private_key=None):
+        """Quantise `values` (torch tensor on any device, numpy array or sequence; float or integer; any shape) with
+        frac_bits fractional bits, pack them on the device and encrypt one ciphertext per slots_per_ciphertext values.
+        `bound` declares max |x|; the slot width leaves room for `headroom` such vectors to be added.  r_values: one r
+        per ciphertext, or None for fresh random r drawn on the device."""
+        torch = _torch()
+        if isinstance(frac_bits, bool) or not isinstance(frac_bits, numbers.Integral) or frac_bits < 0:
+            raise ValueError("frac_bits must be a non-negative integer")
+        if isinstance(headroom, bool) or not isinstance(headroom, numbers.Integral) or headroom < 1:
+            raise ValueError("headroom must be a positive integer")
+        if (isinstance(bound, bool) or not isinstance(bound, numbers.Real) or bound <= 0
+                or not (isinstance(bound, numbers.Integral) or math.isfinite(bound))):
+            raise ValueError("bound must be a positive finite number")
+        frac_bits, headroom = int(frac_bits), int(headroom)
+        qmax = math.ceil(fractions.Fraction(bound) * 2 ** frac_bits)
+        slot_bits = (qmax * headroom).bit_length() + 1
+        if slot_bits > 63:
+            raise ValueError("bound * 2^frac_bits * headroom needs %d-bit slots; at most 63 are supported" % slot_bits)
+        ctx = public_key.engine_context()
+        K = ctx.slots_per_row(slot_bits)
+        device = "cpu" if ctx.eng.simulated else "cuda:%d" % ctx.device
+        q, shape = _quantise(values, bound, frac_bits, device)
+        count = int(q.numel())
+        rows = -(-count // K)
+        if r_values is not None:
+            r_values = list(r_values)
+            if len(r_values) != rows:
+                raise ValueError("%d r_values for %d ciphertexts" % (len(r_values), rows))
+        d_m = torch.empty((rows, ctx.n_limbs), dtype=torch.int32, device=q.device)
+        status = torch.zeros((rows,), dtype=torch.int32, device=q.device)
+        ctx.pack_slots_dev(q, count, slot_bits, d_m, status, stream=_stream(ctx))
+        if bool(status.any().item()):                          # every |q| <= qmax < 2^(slot_bits-1)
+            raise RuntimeError("pack_slots rejected a slot within the bound")
+        rows_enc = EncryptedVector._encrypt_dev_rows(public_key, d_m, np.zeros(rows, dtype=np.int64), r_values, private_key)
+        return cls(rows_enc, shape, slot_bits, frac_bits, qmax)
+
+    # ------------------------------------------------------------------ arithmetic
+    def _result(self, ciphertexts, slot_bound):
+        return PackedEncryptedVector(ciphertexts, self.shape, self.slot_bits, self.frac_bits, slot_bound)
+
+    def _check_bound(self, slot_bound):
+        if slot_bound > _slot_max(self.slot_bits):
+            raise OverflowError("the result's slots could reach %d, beyond the %d-bit slots' %d"
+                                % (slot_bound, self.slot_bits, _slot_max(self.slot_bits)))
+
+    def _check_layout(self, other):
+        if not isinstance(other, PackedEncryptedVector):
+            raise ValueError("a packed vector combines only with a packed vector")
+        if (self.public_key != other.public_key or self.shape != other.shape or self.slot_bits != other.slot_bits
+                or self.frac_bits != other.frac_bits):
+            raise ValueError("packed vectors differ in key, shape, slot_bits or frac_bits")
+
+    def __add__(self, other):
+        if isinstance(other, numbers.Integral) and not isinstance(other, bool) and other == 0:
+            return self                                         # sum() starts from 0
+        if not isinstance(other, (PackedEncryptedVector, EncryptedVector)):
+            return NotImplemented
+        self._check_layout(other)
+        bound = self.slot_bound + other.slot_bound
+        self._check_bound(bound)
+        return self._result(self.ciphertexts + other.ciphertexts, bound)
+
+    __radd__ = __add__
+
+    def __neg__(self):
+        return self * -1
+
+    def __sub__(self, other):
+        if not isinstance(other, (PackedEncryptedVector, EncryptedVector)):
+            return NotImplemented
+        self._check_layout(other)
+        self._check_bound(self.slot_bound + other.slot_bound)
+        return self + (-other)
+
+    def __mul__(self, other):
+        if isinstance(other, (PackedEncryptedVector, EncryptedVector)):
+            raise NotImplementedError('Good luck with that...')
+        if isinstance(other, bool) or not isinstance(other, numbers.Integral):
+            raise TypeError("a packed vector is multiplied by integers only; apply a real factor after decryption")
+        c = int(other)
+        bound = self.slot_bound * abs(c)
+        self._check_bound(bound)
+        return self._result(self.ciphertexts * c, bound)
+
+    __rmul__ = __mul__
+
+    def obfuscate(self):
+        self.ciphertexts.obfuscate()
+
+    # ------------------------------------------------------------------ decryption
+    def decrypt_fixed(self, private_key):
+        """The exact int64 slots (the quantised values, summed and scaled as the operations did), a tensor of .shape on
+        the vector's device.  A ciphertext whose plaintext is not a packing raises ValueError."""
+        if self.public_key != private_key.public_key:
+            raise ValueError('encrypted_number was encrypted against a different key!')
+        torch = _torch()
+        ctx = self.public_key.engine_context()
+        count, rows = len(self), len(self.ciphertexts)
+        dev = self.ciphertexts.limbs.device
+        slots = torch.zeros((count,), dtype=torch.int64, device=dev)
+        if rows:
+            d_m = self.ciphertexts._decrypt_rows_dev(private_key.engine_context())
+            status = torch.zeros((rows,), dtype=torch.int32, device=dev)
+            ctx.unpack_slots_dev(d_m, self.slot_bits, slots, count, status, stream=_stream(ctx))
+            bad = torch.nonzero(status).flatten()
+            if bad.numel():
+                raise ValueError("ciphertext %d does not decrypt to a packing of %d-bit slots" % (int(bad[0]), self.slot_bits))
+        return slots.reshape(self.shape)
+
+    def decrypt(self, private_key):
+        """The values as a float64 tensor of .shape on the vector's device: slot * 2^-frac_bits (exact while |slot| < 2^53)."""
+        return self.decrypt_fixed(private_key).to(_torch().float64) * (2.0 ** -self.frac_bits)
+
+    # ------------------------------------------------------------------ wire format
+    def to_json(self, be_secure=True):
+        """{"packing": {shape, slot_bits, frac_bits, slot_bound}, "ciphertexts": <EncryptedVector.to_json>}"""
+        import json
+        packing = {"shape": list(self.shape), "slot_bits": self.slot_bits, "frac_bits": self.frac_bits,
+                   "slot_bound": self.slot_bound}
+        return '{"packing": %s, "ciphertexts": %s}' % (json.dumps(packing), self.ciphertexts.to_json(be_secure))
+
+    @classmethod
+    def from_json(cls, serialised, public_key=None):
+        import json
+        d = json.loads(serialised)
+        try:
+            p = d["packing"]
+            shape, b, f, bound = p["shape"], p["slot_bits"], p["frac_bits"], p["slot_bound"]
+            cts = d["ciphertexts"]
+        except (KeyError, TypeError) as e:
+            raise ValueError("not a serialised packed vector") from e
+
+        def is_int(x):
+            return isinstance(x, int) and not isinstance(x, bool)
+        if (not isinstance(shape, list) or not all(is_int(x) and x >= 0 for x in shape) or not is_int(b) or not 2 <= b <= 63
+                or not is_int(f) or f < 0 or not is_int(bound) or not 0 <= bound <= _slot_max(b)):
+            raise ValueError("malformed packing layout")
+        if not isinstance(cts, dict):
+            raise ValueError("malformed ciphertexts")
+        try:
+            rows = EncryptedVector.from_json(json.dumps(cts), public_key)
+        except (KeyError, TypeError, IndexError, AttributeError) as e:
+            raise ValueError("malformed ciphertexts") from e
+        K = rows.public_key.engine_context().slots_per_row(b)
+        if len(rows) != -(-math.prod(shape) // K) or rows.exponents.any():
+            raise ValueError("the ciphertexts do not match the packing layout")
+        return cls(rows, shape, b, f, bound)
